@@ -313,8 +313,10 @@ def _blocksparse_prefill_impl(q, kcache, vcache, qscale, kscale, vscale, cu_seql
                  "per-token kscale must be f32 [num_blocks, block_size/32, num_head_kv, 32]")
         _require(vscale.dtype == torch.float32 and vscale.numel() == num_head_kv,
                  "per-head vscale must be f32 [num_head_kv]")
-        args = common[:5] + (_ptr(ks),) + common[6:] + (ks.stride(0), ks.stride(1), ks.stride(2),
-                                                        _stream_of(q))
+        # the stride of a size-1 dim is never applied, and torch may report any value for it
+        # (1 for a contiguous [blocks, 2, 1, 32]); the kernel needs 16-byte multiples
+        kst = tuple(ks.stride(i) if ks.size(i) > 1 else 0 for i in range(3))
+        args = common[:5] + (_ptr(ks),) + common[6:] + kst + (_stream_of(q),)
         _check_rc(_lib.hpc_attention_blocksparse_prefill_qkpertoken_perhead_vperhead_fp8_async(*args),
                   "attention_with_kvcache_blocksparse_prefill_fp8")
     return y
