@@ -595,7 +595,7 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p,
     }
     pp.debug_out = g_dbg_buf[dev];
   }
-  pp.tile_counter = scheduler_counter(stream);  // self-resetting pair of ints, one per stream
+  pp.tile_counter = scheduler_counter(stream);  // self-resetting pair: per stream, or per captured launch
   if (pp.tile_counter == nullptr) return HPC_ERR_CUDA;
   HPC_CUDA_CHECK(launch_pdl(kern, dim3(sm_count()), dim3(kThreads), kSmemBytes, stream, 1, ta, tb, pp));
   return HPC_OK;

@@ -3,6 +3,8 @@
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
+#include <unordered_map>
+#include <vector>
 
 namespace b200 {
 
@@ -42,34 +44,71 @@ int device_slot() {
   return dev < 64 ? dev : 63;
 }
 
-int* scheduler_counter(cudaStream_t stream) {
-  constexpr int kSlots = 128;
-  struct Entry {
-    cudaStream_t stream;
-    bool used;
-  };
-  static int* pool[64] = {nullptr};
-  static Entry table[64][kSlots] = {};
-  static std::mutex mu;
-  const int dev = device_slot();
-  std::lock_guard<std::mutex> lock(mu);
-  if (pool[dev] == nullptr) {
-    if (cudaMalloc(&pool[dev], kSlots * 2 * sizeof(int)) != cudaSuccess ||
-        cudaMemset(pool[dev], 0, kSlots * 2 * sizeof(int)) != cudaSuccess) {
-      set_last_error("scheduler_counter: allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
-      pool[dev] = nullptr;
+namespace {
+
+// Zeroed counter pairs of one device, handed out from chunks that are never moved or freed: a pair
+// may be baked into a CUDA graph that outlives every stream the process has.
+struct CounterPool {
+  std::vector<int*> chunks;
+  int used = 0;  // pairs handed out from the last chunk
+};
+constexpr int kChunkPairs = 1024;
+
+int* new_counter_pair(CounterPool& pool) {
+  if (pool.chunks.empty() || pool.used == kChunkPairs) {
+    // May run while this thread captures a stream. cudaMalloc is not allowed under a global-mode
+    // capture, so this thread switches to relaxed mode for the allocation; the chunk is zeroed on a
+    // private non-blocking stream, so nothing is enqueued on or synchronised with a captured stream.
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    cudaThreadExchangeStreamCaptureMode(&mode);
+    const size_t bytes = kChunkPairs * 2 * sizeof(int);
+    int* p = nullptr;
+    cudaStream_t s = nullptr;
+    cudaError_t e = cudaMalloc(&p, bytes);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaMemsetAsync(p, 0, bytes, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (s != nullptr) cudaStreamDestroy(s);
+    if (e != cudaSuccess && p != nullptr) cudaFree(p);
+    cudaThreadExchangeStreamCaptureMode(&mode);
+    if (e != cudaSuccess) {
+      set_last_error("scheduler_counter: allocation failed: %s", cudaGetErrorString(e));
       return nullptr;
     }
+    pool.chunks.push_back(p);
+    pool.used = 0;
   }
-  int free_slot = -1;
-  for (int i = 0; i < kSlots; i++) {
-    if (table[dev][i].used && table[dev][i].stream == stream) return pool[dev] + 2 * i;
-    if (!table[dev][i].used && free_slot < 0) free_slot = i;
+  return pool.chunks.back() + 2 * pool.used++;
+}
+
+}  // namespace
+
+int* scheduler_counter(cudaStream_t stream) {
+  static CounterPool pools[64];
+  static std::unordered_map<cudaStream_t, int*> by_stream[64];
+  static std::mutex mu;
+  const int dev = device_slot();
+  cudaStreamCaptureStatus status = cudaStreamCaptureStatusNone;
+  const cudaError_t e = cudaStreamIsCapturing(stream, &status);
+  if (e != cudaSuccess) {
+    set_last_error("scheduler_counter: cudaStreamIsCapturing failed: %s", cudaGetErrorString(e));
+    return nullptr;
   }
-  if (free_slot < 0) free_slot = static_cast<int>((reinterpret_cast<uintptr_t>(stream) >> 4) % kSlots);
-  table[dev][free_slot].stream = stream;
-  table[dev][free_slot].used = true;
-  return pool[dev] + 2 * free_slot;
+  std::lock_guard<std::mutex> lock(mu);
+  // A captured launch gets a pair of its own: graphs captured on one stream may be replayed
+  // concurrently on different streams, so the capture stream says nothing about what runs together.
+  if (status == cudaStreamCaptureStatusActive) return new_counter_pair(pools[dev]);
+  // cudaStreamPerThread is one handle value for a different stream on every host thread
+  if (stream == cudaStreamPerThread) {
+    static thread_local int* per_thread[64] = {nullptr};
+    if (per_thread[dev] == nullptr) per_thread[dev] = new_counter_pair(pools[dev]);
+    return per_thread[dev];
+  }
+  auto it = by_stream[dev].find(stream);
+  if (it != by_stream[dev].end()) return it->second;
+  int* p = new_counter_pair(pools[dev]);
+  if (p != nullptr) by_stream[dev].emplace(stream, p);
+  return p;
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,

@@ -38,11 +38,16 @@ bool pdl_enabled();
 // Current CUDA device clamped to [0, 63] (0 when the runtime is unavailable). Launchers keep their
 // one-time state (function attributes, scratch pools) per device: one process may drive several GPUs.
 int device_slot();
-// Two zeroed int32 (work counter, finished-CTA counter) owned by `stream` for kernels that re-arm
-// their scheduler themselves (the last CTA resets both): no memset between launches, so PDL chains
-// and graph replays are unaffected. One slot per (device, stream), allocated and zeroed on first
-// use (not inside a stream capture); launches on one stream are serialised, so the slot is never
-// shared by two running kernels.
+// Two zeroed int32 (work counter, finished-CTA counter) for kernels that re-arm their scheduler
+// themselves (the last CTA resets both): no memset between launches, so PDL chains and graph
+// replays are unaffected. Outside a capture there is one pair per (device, stream) for the life of
+// the process, and one per host thread for cudaStreamPerThread, whose handle value every thread
+// shares. Launches on one stream are serialised (a PDL successor claims work only after its
+// pdl_wait()), so the pair is never used by two running kernels. A stream handle that CUDA reuses
+// after cudaStreamDestroy inherits the pair, which is safe once the old stream's work has finished.
+// A launch being captured into a CUDA graph gets a pair of its own, which the graph keeps; graphs
+// may then be replayed on any streams at once. Safe to call during a capture, including a
+// process's first call.
 int* scheduler_counter(cudaStream_t stream);
 
 // Encode a tiled TMA descriptor (uint8 elements). dims/strides innermost-first; strides in bytes for

@@ -165,7 +165,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       item++;
       if (!alive) {
         // the last CTA out re-arms the work counter for the next launch (no memset node between
-        // launches; one counter pair per stream, see host_utils.h scheduler_counter)
+        // launches; one counter pair per stream or captured launch, see host_utils.h scheduler_counter)
         if (lane == 0) {
           __threadfence();
           if (atomicAdd(p.work_counter + 1, 1) == static_cast<int>(gridDim.x) - 1) {

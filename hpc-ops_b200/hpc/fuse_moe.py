@@ -80,37 +80,60 @@ def _fuse_moe_blockwise_impl(x, x_scale, gate_up_weight, gate_up_weight_scale, d
     _require(down_weight_scale.size(2) == (down_weight.size(2) // 128 + 3) // 4 * 4,
              "down_weight must be per 128 blockwise quant and must be aligned to 4")
     _check_shared(shared_output, x)
+    y = _out(output, x.size(0), x.size(1), x.device)
+    s = _blockwise_scratch(x, gate_up_weight, topk_ids, num_expert_total)
+    _launch_blockwise(y, x, x_scale, gate_up_weight, gate_up_weight_scale, down_weight,
+                      down_weight_scale, topk_ids, topk_scale, shared_output, rank_ep,
+                      num_expert_total, s)
+    return y
 
+
+def _blockwise_scratch(x, gate_up_weight, topk_ids, num_expert_total):
+    """Intermediate tensors of the blockwise pipeline, by stage:
+      route    gate_up_input [rows, H] (gathered x rows, expert-major), gate_up_input_scale
+               [H/128, num_padded] (transposed activation scales, each expert's columns padded to
+               the scale granule), topk_pos, counts, cu_counts, tiles, cu_tiles;
+      Gate-Up  down_input [rows, I] e4m3 and down_input_scale [I/128, num_padded] (same layout);
+      Down     down_output [rows, H] bf16.
+    Also returns num_padded (int)."""
     num_tokens, hidden = x.shape
     num_experts = gate_up_weight.size(0)
-    inter2 = gate_up_weight.size(1)  # 2*I
+    inter = gate_up_weight.size(1) // 2
     num_topk = topk_ids.size(1)
-    avg = num_tokens * num_topk // num_expert_total
-    aligned = _aligned_size(avg)
+    aligned = _aligned_size(num_tokens * num_topk // num_expert_total)
     rows = num_tokens * num_topk
     num_padded = (rows + num_expert_total * aligned + aligned - 1) // aligned * aligned
     dev = x.device
-    y = _out(output, num_tokens, hidden, dev)
     i32 = dict(dtype=torch.int32, device=dev)
-    gate_up_input = torch.empty((rows, hidden), dtype=torch.float8_e4m3fn, device=dev)
-    gate_up_input_scale = torch.empty((x_scale.size(1), num_padded), dtype=torch.float32, device=dev)
-    down_input = torch.empty((rows, inter2 // 2), dtype=torch.float8_e4m3fn, device=dev)
-    down_input_scale = torch.empty((inter2 // 2 // 128, num_padded), dtype=torch.float32, device=dev)
-    down_output = torch.empty((rows, hidden), dtype=torch.bfloat16, device=dev)
-    topk_pos = torch.empty((num_tokens, num_topk), **i32)
-    counts = torch.empty((num_experts,), **i32)
-    cu_counts = torch.empty((num_experts + 1,), **i32)
-    tiles = torch.empty((num_experts,), **i32)
-    cu_tiles = torch.empty((num_experts + 1,), **i32)
+    return dict(
+        gate_up_input=torch.empty((rows, hidden), dtype=torch.float8_e4m3fn, device=dev),
+        gate_up_input_scale=torch.empty((hidden // 128, num_padded), dtype=torch.float32, device=dev),
+        down_input=torch.empty((rows, inter), dtype=torch.float8_e4m3fn, device=dev),
+        down_input_scale=torch.empty((inter // 128, num_padded), dtype=torch.float32, device=dev),
+        down_output=torch.empty((rows, hidden), dtype=torch.bfloat16, device=dev),
+        topk_pos=torch.empty((num_tokens, num_topk), **i32),
+        counts=torch.empty((num_experts,), **i32),
+        cu_counts=torch.empty((num_experts + 1,), **i32),
+        tiles=torch.empty((num_experts,), **i32),
+        cu_tiles=torch.empty((num_experts + 1,), **i32),
+        num_padded=num_padded)
+
+
+def _launch_blockwise(y, x, x_scale, gate_up_weight, gate_up_weight_scale, down_weight,
+                      down_weight_scale, topk_ids, topk_scale, shared_output, rank_ep,
+                      num_expert_total, s):
+    """Enqueue the whole blockwise pipeline with the scratch `s` of _blockwise_scratch."""
+    num_tokens, hidden = x.shape
     _check_rc(_lib.hpc_fuse_moe_blockwise_async(
-        _ptr(y), _ptr(x), _ptr(x_scale), _ptr(gate_up_input), _ptr(gate_up_input_scale), None,
-        _ptr(gate_up_weight), _ptr(gate_up_weight_scale), None, _ptr(down_input),
-        _ptr(down_input_scale), _ptr(down_output), _ptr(down_weight), _ptr(down_weight_scale), None,
-        _ptr(topk_ids), _ptr(topk_scale), _ptr(topk_pos), _ptr(counts), _ptr(cu_counts), _ptr(tiles),
-        _ptr(cu_tiles), _ptr(shared_output), None, None, 0, 0, num_tokens, num_padded, hidden,
-        inter2, num_topk, int(num_expert_total), num_experts, gate_up_weight_scale.size(2),
-        down_weight_scale.size(2), int(rank_ep), _stream_of(x)), "fuse_moe_blockwise")
-    return y
+        _ptr(y), _ptr(x), _ptr(x_scale), _ptr(s["gate_up_input"]), _ptr(s["gate_up_input_scale"]),
+        None, _ptr(gate_up_weight), _ptr(gate_up_weight_scale), None, _ptr(s["down_input"]),
+        _ptr(s["down_input_scale"]), _ptr(s["down_output"]), _ptr(down_weight),
+        _ptr(down_weight_scale), None, _ptr(topk_ids), _ptr(topk_scale), _ptr(s["topk_pos"]),
+        _ptr(s["counts"]), _ptr(s["cu_counts"]), _ptr(s["tiles"]), _ptr(s["cu_tiles"]),
+        _ptr(shared_output), None, None, 0, 0, num_tokens, s["num_padded"], hidden,
+        gate_up_weight.size(1), topk_ids.size(1), int(num_expert_total), gate_up_weight.size(0),
+        gate_up_weight_scale.size(2), down_weight_scale.size(2), int(rank_ep), _stream_of(x)),
+        "fuse_moe_blockwise")
 
 
 def _fuse_moe_impl(x, gate_up_weight, down_weight, gate_up_scale, down_scale, act_and_mul_scale,
