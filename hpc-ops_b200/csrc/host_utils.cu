@@ -58,8 +58,9 @@ struct CounterPool {
 };
 constexpr int kChunkPairs = 1024;
 
-int* new_counter_pair(CounterPool& pool) {
-  if (pool.chunks.empty() || pool.used == kChunkPairs) {
+// `pairs` consecutive pairs; kChunkPairs is a multiple of every `pairs` a pool is used with.
+int* new_counter_pair(CounterPool& pool, int pairs = 1) {
+  if (pool.chunks.empty() || pool.used + pairs > kChunkPairs) {
     // May run while this thread captures a stream. cudaMalloc is not allowed under a global-mode
     // capture, so this thread switches to relaxed mode for the allocation; the chunk is zeroed on a
     // private non-blocking stream, so nothing is enqueued on or synchronised with a captured stream.
@@ -82,37 +83,62 @@ int* new_counter_pair(CounterPool& pool) {
     pool.chunks.push_back(p);
     pool.used = 0;
   }
-  return pool.chunks.back() + 2 * pool.used++;
+  int* p = pool.chunks.back() + 2 * pool.used;
+  pool.used += pairs;
+  return p;
 }
+
+// Per-stream device storage of `kPairs` zeroed pairs, handed out as scheduler_counter describes.
+// Every block handed out gets the next serial number (1, 2, ...) of its table.
+template <int kPairs>
+struct StreamTable {
+  struct Entry {
+    int* p = nullptr;
+    uint64_t serial = 0;
+  };
+  CounterPool pools[64];
+  std::unordered_map<cudaStream_t, Entry> by_stream[64];
+  std::mutex mu;
+  uint64_t handed_out = 0;
+
+  int* get(cudaStream_t stream, uint64_t* serial) {
+    const int dev = device_slot();
+    cudaStreamCaptureStatus status = cudaStreamCaptureStatusNone;
+    const cudaError_t e = cudaStreamIsCapturing(stream, &status);
+    if (e != cudaSuccess) {
+      set_last_error("scheduler_counter: cudaStreamIsCapturing failed: %s", cudaGetErrorString(e));
+      return nullptr;
+    }
+    std::lock_guard<std::mutex> lock(mu);
+    Entry fresh;
+    Entry* slot = &fresh;
+    // A captured launch gets a block of its own: graphs captured on one stream may be replayed
+    // concurrently on different streams, so the capture stream says nothing about what runs together.
+    if (status != cudaStreamCaptureStatusActive) {
+      // cudaStreamPerThread is one handle value for a different stream on every host thread
+      static thread_local Entry per_thread[64];
+      slot = stream == cudaStreamPerThread ? &per_thread[dev] : &by_stream[dev][stream];
+    }
+    if (slot->p == nullptr) {
+      slot->p = new_counter_pair(pools[dev], kPairs);
+      if (slot->p == nullptr) return nullptr;
+      slot->serial = ++handed_out;
+    }
+    if (serial != nullptr) *serial = slot->serial;
+    return slot->p;
+  }
+};
 
 }  // namespace
 
 int* scheduler_counter(cudaStream_t stream) {
-  static CounterPool pools[64];
-  static std::unordered_map<cudaStream_t, int*> by_stream[64];
-  static std::mutex mu;
-  const int dev = device_slot();
-  cudaStreamCaptureStatus status = cudaStreamCaptureStatusNone;
-  const cudaError_t e = cudaStreamIsCapturing(stream, &status);
-  if (e != cudaSuccess) {
-    set_last_error("scheduler_counter: cudaStreamIsCapturing failed: %s", cudaGetErrorString(e));
-    return nullptr;
-  }
-  std::lock_guard<std::mutex> lock(mu);
-  // A captured launch gets a pair of its own: graphs captured on one stream may be replayed
-  // concurrently on different streams, so the capture stream says nothing about what runs together.
-  if (status == cudaStreamCaptureStatusActive) return new_counter_pair(pools[dev]);
-  // cudaStreamPerThread is one handle value for a different stream on every host thread
-  if (stream == cudaStreamPerThread) {
-    static thread_local int* per_thread[64] = {nullptr};
-    if (per_thread[dev] == nullptr) per_thread[dev] = new_counter_pair(pools[dev]);
-    return per_thread[dev];
-  }
-  auto it = by_stream[dev].find(stream);
-  if (it != by_stream[dev].end()) return it->second;
-  int* p = new_counter_pair(pools[dev]);
-  if (p != nullptr) by_stream[dev].emplace(stream, p);
-  return p;
+  static StreamTable<1> table;
+  return table.get(stream, nullptr);
+}
+
+int* stream_state(cudaStream_t stream, uint64_t* serial) {
+  static StreamTable<2> table;
+  return table.get(stream, serial);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,

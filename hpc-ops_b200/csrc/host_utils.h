@@ -46,6 +46,10 @@ bool pdl_enabled();
 // may then be replayed on any streams at once. Safe to call during a capture, including a
 // process's first call.
 int* scheduler_counter(cudaStream_t stream);
+// Sixteen zeroed bytes (two pairs, 8-byte aligned) handed out exactly as scheduler_counter, from a
+// table of their own, for state a kernel keeps across launches on one stream. `*serial` (if not
+// null) receives the block's number, unique in the process and the same on every call for a stream.
+int* stream_state(cudaStream_t stream, uint64_t* serial);
 
 // Encode a tiled TMA descriptor (uint8 elements). dims/strides innermost-first; strides in bytes for
 // dims 1..rank-1. Returns 0 on success.

@@ -100,12 +100,23 @@ lib.hpc_attention_blocksparse_prefill_qkpertoken_perhead_vperhead_fp8_async.argt
     _prefill_args + [c_i64] * 3 + [c_ptr])
 
 # (hasattr: a library built from an older commit, e.g. for an A/B timing, lacks these symbols; it
-# still fails loudly -- at the first rope call)
+# still fails loudly -- at the first rope or sampler call)
 if hasattr(lib, "hpc_rope_norm_store_kv_async"):
     lib.hpc_rope_norm_store_kv_async.restype = c_int
     lib.hpc_rope_norm_store_kv_async.argtypes = [c_ptr] * 12 + [c_int] * 12 + [c_ptr]
     lib.hpc_rope_norm_store_kv_fp8_async.restype = c_int
     lib.hpc_rope_norm_store_kv_fp8_async.argtypes = [c_ptr] * 17 + [c_f32] + [c_int] * 14 + [c_ptr]
+
+if hasattr(lib, "hpc_fused_sampler_async"):
+    lib.hpc_fused_sampler_async.restype = c_int
+    lib.hpc_fused_sampler_async.argtypes = (
+        [c_ptr, c_ptr, c_i64, c_int, c_int, c_int, c_ptr, c_i64, c_ptr, c_ptr, c_f32, c_ptr, c_f32,
+         c_int, c_ptr, c_int, c_int, c_ptr, c_f32, c_int, c_ptr, ctypes.c_uint64, c_ptr])
+    lib.hpc_fused_sampler_temperature_sample_async.restype = c_int
+    lib.hpc_fused_sampler_temperature_sample_async.argtypes = (
+        [c_ptr, c_ptr, c_i64, c_int, c_int, c_int, c_ptr, c_f32, c_ptr, c_ptr, ctypes.c_uint64, c_ptr])
+    lib.hpc_sampler_rng_offset.restype = c_int
+    lib.hpc_sampler_rng_offset.argtypes = [c_ptr, ctypes.POINTER(ctypes.c_uint64)]
 
 
 def check(rc: int, what: str = ""):

@@ -323,6 +323,32 @@ int hpc_rope_norm_store_kv_fp8_async(
     int kv_block_size, int num_rows, int num_q_heads, int num_kv_heads, int qk_head_dim,
     int v_head_dim, int is_prefill, int qk_norm_policy, int quant_policy, cudaStream_t stream);
 
+/* ---- fused sampler ---------------------------------------------------------------------------
+ * replaces reference src/sampler/entry.cc (fused_sampler, fused_sampler_temperature_sample).
+ * logits [batch, vocab] fp32 (dtype 0) or bf16 (dtype 1), `row_stride` elements between rows, rows
+ * 16-byte aligned, vocab % 8 == 0 and max_topk <= vocab <= 262144; out: int32 [batch].
+ * Per-row parameters are a [batch] array or, when the pointer is null, the scalar `*_val`; topk is
+ * int32 or int64 (topk_is_int64). penalty_mask [*, mask_stride] uint8, one bit per token, read
+ * at row slot_id[b]; the sampled token's bit is set with an atomicOr on the aligned 4-byte word
+ * holding it, so the mask must start 4-byte aligned and span a multiple of 4 bytes. gumbel_noise [batch, vocab]
+ * fp32 contiguous, or null: then Philox4x32-10 noise keyed by `seed` (> 0) is drawn in the kernel.
+ */
+int hpc_fused_sampler_async(
+    int* out, const void* logits, int64_t row_stride, int dtype, int batch, int vocab,
+    uint8_t* penalty_mask, int64_t mask_stride, const int* slot_id, const float* repetition_penalty,
+    float repetition_penalty_val, const float* temperature, float temperature_val,
+    int softmax_policy, const void* topk, int topk_is_int64, int topk_val, const float* topp,
+    float topp_val, int max_topk, const float* gumbel_noise, uint64_t seed, cudaStream_t stream);
+/* temperature-only Gumbel-max; rows with temperature <= 0 (or NaN) take the argmax of the logits.
+ * draft_token_ids [batch] int64 or null: that token of row b scores -inf when in [0, vocab). */
+int hpc_fused_sampler_temperature_sample_async(
+    int* out, const void* logits, int64_t row_stride, int dtype, int batch, int vocab,
+    const float* temperature, float temperature_val, const float* gumbel_noise,
+    const int64_t* draft_token_ids, uint64_t seed, cudaStream_t stream);
+/* The Philox launch offset the next sampler launch on `stream` will use (synchronises `stream`).
+ * For tests: the internal noise of that launch is then known to the caller. */
+int hpc_sampler_rng_offset(cudaStream_t stream, uint64_t* offset);
+
 #ifdef __cplusplus
 }
 #endif
