@@ -100,12 +100,19 @@ lib.hpc_attention_blocksparse_prefill_qkpertoken_perhead_vperhead_fp8_async.argt
     _prefill_args + [c_i64] * 3 + [c_ptr])
 
 # (hasattr: a library built from an older commit, e.g. for an A/B timing, lacks these symbols; it
-# still fails loudly -- at the first rope or sampler call)
+# still fails loudly -- at the first rope, sampler or bf16 prefill call)
 if hasattr(lib, "hpc_rope_norm_store_kv_async"):
     lib.hpc_rope_norm_store_kv_async.restype = c_int
     lib.hpc_rope_norm_store_kv_async.argtypes = [c_ptr] * 12 + [c_int] * 12 + [c_ptr]
     lib.hpc_rope_norm_store_kv_fp8_async.restype = c_int
     lib.hpc_rope_norm_store_kv_fp8_async.argtypes = [c_ptr] * 17 + [c_f32] + [c_int] * 14 + [c_ptr]
+
+if hasattr(lib, "hpc_attention_prefill_bf16_async"):
+    lib.hpc_attention_prefill_bf16_async.restype = c_int
+    lib.hpc_attention_prefill_bf16_async.argtypes = [c_ptr] * 6 + [c_int] * 11 + [c_ptr]
+    lib.hpc_attention_with_kvcache_prefill_bf16_async.restype = c_int
+    lib.hpc_attention_with_kvcache_prefill_bf16_async.argtypes = (
+        [c_ptr] * 7 + [c_int] * 12 + [c_i64] * 6 + [c_ptr])
 
 if hasattr(lib, "hpc_fused_sampler_async"):
     lib.hpc_fused_sampler_async.restype = c_int

@@ -5,6 +5,9 @@ Implemented in this build (sm_90a):
                                       QPERTOKEN_PERHEAD_KPERTOKEN_PERHEAD_VPERHEAD (in-cache k scales)
   * attention_decode_bf16           — pages of 16 / 32 / 64 tokens, mtp 0..4
   * attention_with_kvcache_blocksparse_prefill_fp8 / attention_with_kvcache_prefill_fp8 (dense)
+  * attention_prefill_bf16 (varlen causal self-attention on contiguous q/k/v) and
+    attention_with_kvcache_prefill_bf16 (causal, chunked, prefill over the paged bf16 cache,
+    pages of 16 / 32 / 64 tokens)
   * get_attention_decode_task_workspace / assign_attention_decode_task (CPU and CUDA)
   * print_attention_decode_task
 The host side does what the reference's torch entry does (validation, scratch allocation, stride
@@ -345,6 +348,98 @@ _ops.define(
     "Tensor? output) -> (Tensor)")
 _ops.impl("attention_with_kvcache_prefill_fp8", _dense_prefill_fp8_impl, "CUDA")
 
+def _bf16_prefill_common(who, q, output, index_tensors):
+    """Checks shared by the two bf16 prefill ops; returns (total_seq, num_head_q, y)."""
+    _require(q.is_cuda, "q tensor must be cuda")
+    for t, name in index_tensors:
+        _require(t.is_cuda, f"{name} tensor must be cuda")
+        _require(t.dtype == torch.int32 and t.is_contiguous(), f"{name} must be contiguous int32")
+    _require(q.dtype == torch.bfloat16, "q dtype must be bfloat16")
+    _require(q.dim() == 3 and q.size(2) == 128, f"{who}: head dim must be 128")
+    _require(q.stride(2) == 1 and q.stride(1) == 128, "q must be contiguous in (head, dim)")
+    total_seq, num_head_q = q.size(0), q.size(1)
+    if output is not None:
+        _require(output.is_cuda and output.device == q.device, "output tensor must be cuda, on q's device")
+        _require(output.dtype == torch.bfloat16, "output dtype must be bfloat16")
+        _require(output.is_contiguous(), "output tensor must be contiguous")
+        _require(tuple(output.shape) == (total_seq, num_head_q, 128),
+                 "output must have shape [total_seq_q, num_head_q, 128]")
+        y = output
+    else:
+        y = torch.empty((total_seq, num_head_q, 128), dtype=torch.bfloat16, device=q.device)
+    return total_seq, num_head_q, y
+
+
+def _attention_prefill_bf16_impl(q, k, v, seqlens_q, cu_seqlens_q, max_seqlens_q, output=None):
+    """Varlen causal self-attention on contiguous bf16 q/k/v; validation follows reference
+    src/attention/entry.cc:15-70."""
+    who = "attention_prefill_bf16"
+    total_seq, num_head_q, y = _bf16_prefill_common(
+        who, q, output, ((seqlens_q, "seqlens_q"), (cu_seqlens_q, "cu_seqlens_q")))
+    _require(k.is_cuda and v.is_cuda, "k and v tensors must be cuda")
+    _require(k.dtype == torch.bfloat16 and v.dtype == torch.bfloat16, "k and v dtype must be bfloat16")
+    _require(k.dim() == 3 and v.dim() == 3 and k.size(2) == 128 and v.size(2) == 128,
+             f"{who}: head dim must be 128")
+    _require(k.size(0) == total_seq and v.size(0) == total_seq and k.size(1) == v.size(1),
+             "k and v must be [total_seq_q, num_head_kv, 128]")
+    _require(k.stride(2) == 1 and k.stride(1) == 128 and v.stride(2) == 1 and v.stride(1) == 128,
+             "k and v must be contiguous in (head, dim)")
+    num_head_kv = k.size(1)
+    _require(num_head_kv > 0 and num_head_q % num_head_kv == 0,
+             "num_head_q must be a multiple of num_head_kv")
+    num_batch = seqlens_q.size(0)
+    _require(cu_seqlens_q.numel() == num_batch + 1, "cu_seqlens_q must have num_batch + 1 entries")
+    _check_rc(_lib.hpc_attention_prefill_bf16_async(
+        _ptr(y), _ptr(q), _ptr(k), _ptr(v), _ptr(seqlens_q), _ptr(cu_seqlens_q), num_batch,
+        total_seq, int(max_seqlens_q), 128, 128, num_head_q, num_head_kv, y.stride(0), q.stride(0),
+        k.stride(0), v.stride(0), _stream_of(q)), who)
+    return y
+
+
+def _attention_with_kvcache_prefill_bf16_impl(q, kcache, vcache, cu_seqlens_q, block_ids,
+                                              seqlens_kvcache, max_seqlens_q, output=None):
+    """Causal (chunked) prefill over the paged bf16 KV cache; validation follows reference
+    src/attention/entry.cc:72-150."""
+    who = "attention_with_kvcache_prefill_bf16"
+    total_seq, num_head_q, y = _bf16_prefill_common(
+        who, q, output, ((cu_seqlens_q, "cu_seqlens_q"), (block_ids, "block_ids"),
+                         (seqlens_kvcache, "seqlens_kvcache")))
+    _require(kcache.is_cuda and vcache.is_cuda, "kv cache tensors must be cuda")
+    _require(kcache.dtype == torch.bfloat16 and vcache.dtype == torch.bfloat16,
+             "kcache and vcache dtype must be bfloat16")
+    _require(kcache.dim() == 4 and kcache.shape == vcache.shape,
+             "kcache and vcache must both be [num_blocks, block_size, num_head_kv, 128]")
+    _require(kcache.size(3) == 128, f"{who}: head dim must be 128")
+    _require(kcache.stride(3) == 1 and vcache.stride(3) == 1, "kv cache innermost dim must be contiguous")
+    num_blocks, block_size, num_head_kv = kcache.size(0), kcache.size(1), kcache.size(2)
+    _require(block_size in (16, 32, 64), "kvcache paged blocksize must be 16, 32 or 64.")
+    _require(num_head_q % num_head_kv == 0, "num_head_q must be a multiple of num_head_kv")
+    num_batch = cu_seqlens_q.numel() - 1
+    _require(num_batch > 0 and seqlens_kvcache.numel() == num_batch
+             and block_ids.dim() == 2 and block_ids.size(0) == num_batch,
+             "cu_seqlens_q [B+1], seqlens_kvcache [B] and block_ids [B, max_blocks] disagree on B")
+    _check_rc(_lib.hpc_attention_with_kvcache_prefill_bf16_async(
+        _ptr(y), _ptr(q), _ptr(kcache), _ptr(vcache), _ptr(cu_seqlens_q), _ptr(block_ids),
+        _ptr(seqlens_kvcache), num_batch, total_seq, int(max_seqlens_q), 128, 128, num_head_q,
+        num_head_kv, num_blocks, block_size, block_ids.size(1), y.stride(0), q.stride(0),
+        kcache.stride(0), kcache.stride(1), kcache.stride(2),
+        vcache.stride(0), vcache.stride(1), vcache.stride(2), _stream_of(q)), who)
+    return y
+
+
+# schemas of reference src/attention/entry.cc (attention_prefill_bf16,
+# attention_with_kvcache_prefill_bf16 registrations)
+_ops.define(
+    "attention_prefill_bf16(Tensor q, Tensor k, Tensor v, Tensor seqlens_q, Tensor cu_seqlens_q, "
+    "int max_seqlens_q, Tensor? output) -> (Tensor)")
+_ops.impl("attention_prefill_bf16", _attention_prefill_bf16_impl, "CUDA")
+
+_ops.define(
+    "attention_with_kvcache_prefill_bf16(Tensor q, Tensor kcache, Tensor vcache,"
+    "Tensor cu_seqlens_q, Tensor block_ids, Tensor num_seq_kvcache, int max_seqlens_q, "
+    "Tensor? output) -> (Tensor)")
+_ops.impl("attention_with_kvcache_prefill_bf16", _attention_with_kvcache_prefill_bf16_impl, "CUDA")
+
 _ops.define(
     "attention_decode_bf16(Tensor q, Tensor! kcache, Tensor! vcache, Tensor block_ids, Tensor "
     "num_seq_kvcache, int mtp, bool new_kv_included, bool use_splitk, Tensor? task_map, "
@@ -421,6 +516,55 @@ def attention_with_kvcache_blocksparse_prefill_fp8(
     return torch.ops.hpc.attention_with_kvcache_blocksparse_prefill_fp8(
         q, kcache, vcache, qscale, kscale, vscale, cu_seqlens_q, block_ids, seqlens_kvcache,
         max_seqlens_q, quant_type.value, block_mask, output)
+
+
+def attention_prefill_bf16(
+    q: Tensor,
+    k: Tensor,
+    v: Tensor,
+    seqlens_q: Tensor,
+    cu_seqlens_q: Tensor,
+    max_seqlens_q: int,
+    output: Tensor = None,
+) -> Tensor:
+    """Varlen causal self-attention in bf16 (contract of reference hpc/attention.py:15-64):
+    softmax(Q K^T / sqrt(128)) V per request, query i seeing keys 0..i of its own request.
+
+      q           [total_seq, num_head_q, 128] bfloat16, contiguous in (head, dim)
+      k, v        [total_seq, num_head_kv, 128] bfloat16, same; num_head_q % num_head_kv == 0
+      seqlens_q   [num_batch] int32, equal to the lengths cu_seqlens_q gives
+      cu_seqlens_q [num_batch + 1] int32: request b is rows cu_seqlens_q[b] .. cu_seqlens_q[b+1]-1
+      max_seqlens_q  at least the longest request (a larger value only costs idle work items)
+      output      optional contiguous bf16 [total_seq, num_head_q, 128]
+    Returns bf16 [total_seq, num_head_q, 128]."""
+    return torch.ops.hpc.attention_prefill_bf16(q, k, v, seqlens_q, cu_seqlens_q, max_seqlens_q,
+                                                output)
+
+
+def attention_with_kvcache_prefill_bf16(
+    q: Tensor,
+    kcache: Tensor,
+    vcache: Tensor,
+    cu_seqlens_q: Tensor,
+    block_ids: Tensor,
+    seqlens_kvcache: Tensor,
+    max_seqlens_q: int,
+    output: Tensor = None,
+) -> Tensor:
+    """Causal prefill, including chunked prefill, over the paged bf16 KV cache (contract of
+    reference hpc/attention.py:67-145): the `sq` new tokens of request b are the last ones of its
+    `skv = seqlens_kvcache[b]` cached tokens, and new token i sees cached keys j <= skv - sq + i.
+
+      q           [total_seq, num_head_q, 128] bfloat16, contiguous in (head, dim)
+      kcache, vcache [num_blocks, block_size, num_head_kv, 128] bfloat16, block_size 16 / 32 / 64,
+                  any strides on dims 0-2 (NHD or HND). Slots past skv in a request's last page are
+                  never read into the result, whatever they hold.
+      cu_seqlens_q [num_batch + 1] int32; block_ids [num_batch, max_blocks] int32;
+      seqlens_kvcache [num_batch] int32 (cached tokens including the new ones)
+      output      optional contiguous bf16 [total_seq, num_head_q, 128]
+    Returns bf16 [total_seq, num_head_q, 128]. Requests with sq = 0 write nothing."""
+    return torch.ops.hpc.attention_with_kvcache_prefill_bf16(
+        q, kcache, vcache, cu_seqlens_q, block_ids, seqlens_kvcache, max_seqlens_q, output)
 
 
 def attention_decode_bf16(
@@ -637,6 +781,22 @@ def _attention_decode_fp8_fake(
     q, kcache, vcache, block_ids, num_seq_kvcache, qscale, kscale, vscale, mtp, new_kv_included,
     quant_type, use_splitk, task_map, split_flag, output,
 ):
+    if output is not None:
+        return output
+    return torch.empty((q.size(0), q.size(1), vcache.size(3)), dtype=torch.bfloat16,
+                       device=q.device)
+
+
+@torch.library.register_fake("hpc::attention_prefill_bf16")
+def _attention_prefill_bf16_fake(q, k, v, seqlens_q, cu_seqlens_q, max_seqlens_q, output=None):
+    if output is not None:
+        return output
+    return torch.empty((q.size(0), q.size(1), v.size(2)), dtype=torch.bfloat16, device=q.device)
+
+
+@torch.library.register_fake("hpc::attention_with_kvcache_prefill_bf16")
+def _attention_with_kvcache_prefill_bf16_fake(q, kcache, vcache, cu_seqlens_q, block_ids,
+                                              num_seq_kvcache, max_seqlens_q, output=None):
     if output is not None:
         return output
     return torch.empty((q.size(0), q.size(1), vcache.size(3)), dtype=torch.bfloat16,

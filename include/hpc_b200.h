@@ -298,6 +298,34 @@ int hpc_attention_blocksparse_prefill_qkpertoken_perhead_vperhead_fp8_async(
     int64_t k_head, int64_t v_blk, int64_t v_tok, int64_t v_head, int64_t ks_blk, int64_t ks_grp,
     int64_t ks_head, cudaStream_t stream);
 
+/* ---- BF16 causal prefill --------------------------------------------------------------------------
+ * replace reference src/attention/prefill/prefill.h:12-25 without the `tmas` scratch. Head dim 128
+ * for qk and v, num_head_q % num_head_kv == 0, softmax scale 1/sqrt(128), causal mask aligned to
+ * the bottom right (query i of a request with sq new and skv total tokens sees keys
+ * j <= skv - sq + i, and no key j >= skv). Out bf16 [total_seq_q, Hq, 128], ldY = token stride;
+ * rows of requests with sq = 0 are not written. Strides in elements, multiples of 8; q, k, v, out
+ * are 16-byte aligned with heads 128 elements apart within a token.
+ * Dense: q [total_seq_q, Hq, 128], k / v [total_seq_q, Hkv, 128] (token strides ldQ / ldK / ldV);
+ *   request b is rows cu_seqlens_q[b] .. cu_seqlens_q[b + 1] - 1 of each, attending to itself;
+ *   seqlens_q[b] must equal its length.
+ * Paged: caches [blocks, block_size, Hkv, 128], block_size 16 / 32 / 64, strides (blk, tok, head)
+ *   = (ldK, ldK1, ldK2) and (ldV, ldV1, ldV2), NHD or HND; block_ids [B, num_seq_max_blocks];
+ *   seqlens_kvcache [B] = cached tokens including the new ones.
+ */
+int hpc_attention_prefill_bf16_async(void* y_ptr, const void* q_ptr, const void* k_ptr,
+                                     const void* v_ptr, const int* seqlens_q_ptr,
+                                     const int* cu_seqlens_q_ptr, int num_batch, int total_seq_q,
+                                     int max_seq_q, int num_dim_qk, int num_dim_v, int num_head_q,
+                                     int num_head_kv, int ldY, int ldQ, int ldK, int ldV,
+                                     cudaStream_t stream);
+int hpc_attention_with_kvcache_prefill_bf16_async(
+    void* y_ptr, const void* q_ptr, const void* kcache_ptr, const void* vcache_ptr,
+    const int* cu_seqlens_q_ptr, const int* block_ids_ptr, const int* seqlens_kvcache_ptr,
+    int num_batch, int total_seq_q, int max_seq_q, int num_dim_qk, int num_dim_v, int num_head_q,
+    int num_head_kv, int num_kvcache_blocks, int block_size, int num_seq_max_blocks, int ldY,
+    int ldQ, int64_t ldK, int64_t ldK1, int64_t ldK2, int64_t ldV, int64_t ldV1, int64_t ldV2,
+    cudaStream_t stream);
+
 /* ---- RoPE + QK RMSNorm + paged KV-cache store (the producer of the cache layout attention reads) --
  * replaces reference src/rope/rope.h:15-25 (rope_norm_store_kv_async) and :27-38
  * (rope_norm_store_kv_fp8_async), argument for argument (bool -> int). Cache pages are

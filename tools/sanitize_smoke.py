@@ -1,5 +1,5 @@
-"""One small invocation of every hot-path op (decode both quant types, prefill both, blockwise +
-per-tensor MoE, route GEMM, W=1 allreduce, rope), meant to run under compute-sanitizer:
+"""One small invocation of every hot-path op (decode both quant types, prefill both, bf16 prefill
+dense and paged, blockwise + per-tensor MoE, route GEMM, W=1 allreduce, rope), meant to run under compute-sanitizer:
 
     compute-sanitizer --tool memcheck  python tools/sanitize_smoke.py
     compute-sanitizer --tool synccheck python tools/sanitize_smoke.py
@@ -25,7 +25,8 @@ def cuda(d):
 
 
 def main():
-    which = set(sys.argv[1:]) or {"decode", "prefill", "moe", "gemm", "allreduce", "rope"}
+    which = set(sys.argv[1:]) or {"decode", "prefill", "prefill_bf16", "moe", "gemm", "allreduce",
+                                  "rope"}
     if "decode" in which:
         B, hkv, hq = 3, 2, 8
         lens = [300, 129, 64]
@@ -64,6 +65,22 @@ def main():
                                         d["block_mask"], kpt)
             assert torch.allclose(y.float().cpu(), gt.float(), atol=0.1)
         print("prefill ok")
+    if "prefill_bf16" in which:
+        from oracle import prefill_bf16 as ob
+        from synth import prefill_bf16 as sb
+        for case in (sb.GRID[0], sb.GRID[3]):  # dense; paged with 16-token pages and an sq = 0 slot
+            d = sb.make_exact_case(case, "needle", device="cuda")
+            if d["op"] == "dense":
+                y = hpc.attention_prefill_bf16(d["q"], d["k"], d["v"], d["seqlens_q"],
+                                               d["cu_seqlens_q"], d["max_q"])
+            else:
+                y = hpc.attention_with_kvcache_prefill_bf16(d["q"], d["kcache"], d["vcache"],
+                                                            d["cu_seqlens_q"], d["block_ids"],
+                                                            d["seqlens_kv"], d["max_q"])
+            r = ob.check(y.cpu(), {k: (v.cpu() if isinstance(v, torch.Tensor) else v)
+                                   for k, v in d.items()})
+            assert r["ok_a"] and r["ok_b"], r
+        print("prefill_bf16 ok")
     if "moe" in which:
         d = om.make_moe_blockwise_inputs(96, 4, 256, 256, 8, 1, False, seed=5)
         c = cuda(d)
