@@ -125,6 +125,22 @@ if hasattr(lib, "hpc_fused_sampler_async"):
     lib.hpc_sampler_rng_offset.restype = c_int
     lib.hpc_sampler_rng_offset.argtypes = [c_ptr, ctypes.POINTER(ctypes.c_uint64)]
 
+if hasattr(lib, "hpc_stem_tpd_async"):
+    lib.hpc_stem_oam_prep_paged_kv_qpertoken_perhead_kvpertensor_dim128_async.restype = c_int
+    lib.hpc_stem_oam_prep_paged_kv_qpertoken_perhead_kvpertensor_dim128_async.argtypes = (
+        [c_ptr] * 8 + [c_int] * 9 + [c_f32, c_int, c_int] + [c_i64] * 6 + [c_ptr, c_ptr])
+    lib.hpc_stem_oam_prep_paged_kv_qkpertoken_perhead_vperhead_dim128_async.restype = c_int
+    lib.hpc_stem_oam_prep_paged_kv_qkpertoken_perhead_vperhead_dim128_async.argtypes = (
+        [c_ptr] * 8 + [c_int] * 10 + [c_f32, c_int, c_int] + [c_i64] * 9 + [c_ptr, c_ptr])
+    lib.hpc_stem_oam_prep_varlen_q_dim128_async.restype = c_int
+    lib.hpc_stem_oam_prep_varlen_q_dim128_async.argtypes = (
+        [c_ptr] * 5 + [c_int] * 6 + [c_i64] * 3 + [c_ptr])
+    lib.hpc_stem_oam_gemm_dim128_async.restype = c_int
+    lib.hpc_stem_oam_gemm_dim128_async.argtypes = [c_ptr] * 6 + [c_int] * 8 + [c_ptr]
+    lib.hpc_stem_tpd_async.restype = c_int
+    lib.hpc_stem_tpd_async.argtypes = (
+        [c_ptr] * 5 + [c_int] * 5 + [c_f32, c_int, c_int, c_f32, c_int, c_f32, c_int, c_ptr])
+
 
 def check(rc: int, what: str = ""):
     """Turn a launcher status into the RuntimeError the reference raises via TORCH_CHECK."""

@@ -377,6 +377,56 @@ int hpc_fused_sampler_temperature_sample_async(
  * For tests: the internal noise of that launch is then known to the caller. */
 int hpc_sampler_rng_offset(cudaStream_t stream, uint64_t* offset);
 
+/* ---- Stem block-mask generation (block-sparse FP8 prefill) ----------------------------------
+ * replaces reference src/stem/*.h, argument for argument (bool -> int), with cache and scale
+ * strides added. Only stem_block_size 128, stem_stride 16 and head dim 128.
+ * prep_paged_kv: caches [blocks, page (32 or 64), Hkv, 128] e4m3 read through ldK/ldV (block),
+ * ldK1/ldV1 (token) and ldK2/ldV2 (head) strides in elements, so NHD and HND both work;
+ * kflat [B, Hkv, max_num_stem_blocks, 2048] bf16, vbias [B, Hkv, max_num_stem_blocks] fp32,
+ * v_norm_down [B, Hkv, max_k_down_len = 8 * max_num_stem_blocks] fp32 scratch. Blocks past a
+ * request's ceil(kv / 128) are not written. quant "kvpertensor": kscale, vscale [1] fp32;
+ * "qkpertoken_perhead_vperhead": kscale [blocks, page / 32, Hkv, 32] fp32 (ldKS, ldKS1, ldKS2 in
+ * fp32 elements), vscale [Hkv].
+ */
+int hpc_stem_oam_prep_paged_kv_qpertoken_perhead_kvpertensor_dim128_async(
+    void* kflat_ptr, void* vbias_ptr, const void* kcache_ptr, const void* vcache_ptr,
+    const void* kscale_ptr, const void* vscale_ptr, const void* block_ids_ptr,
+    const void* kv_seq_lens_ptr, int num_batch, int num_dim_qk, int num_dim_v, int num_head_kv,
+    int num_kvcache_blocks, int block_size, int num_seq_max_blocks, int stem_block_size,
+    int stem_stride, float lambda_mag, int max_num_stem_blocks, int max_k_down_len, int64_t ldK,
+    int64_t ldV, int64_t ldK1, int64_t ldK2, int64_t ldV1, int64_t ldV2, void* v_norm_down_ptr,
+    cudaStream_t stream);
+int hpc_stem_oam_prep_paged_kv_qkpertoken_perhead_vperhead_dim128_async(
+    void* kflat_ptr, void* vbias_ptr, const void* kcache_ptr, const void* vcache_ptr,
+    const void* kscale_ptr, const void* vscale_ptr, const void* block_ids_ptr,
+    const void* kv_seq_lens_ptr, int num_batch, int num_dim_qk, int num_dim_v, int num_head_kv,
+    int num_kvcache_blocks, int block_size, int scale_block_size, int num_seq_max_blocks,
+    int stem_block_size, int stem_stride, float lambda_mag, int max_num_stem_blocks,
+    int max_k_down_len, int64_t ldK, int64_t ldV, int64_t ldKS, int64_t ldKS1, int64_t ldKS2,
+    int64_t ldK1, int64_t ldK2, int64_t ldV1, int64_t ldV2, void* v_norm_down_ptr,
+    cudaStream_t stream);
+/* q_fp8 [total, Hq, 128] e4m3 (ldQ elements between tokens), qscale [B, Hq, >= max q] fp32 read
+ * through its strides ldQS, ldQS1, ldQS2 (elements); qflat [B, Hq, max_num_q_blocks, 2048] bf16. */
+int hpc_stem_oam_prep_varlen_q_dim128_async(
+    void* qflat_ptr, const void* q_fp8_ptr, const void* qscale_ptr, const void* q_seq_lens_ptr,
+    const void* cu_seqlens_q_ptr, int num_batch, int num_head_q, int ldQ, int stem_block_size,
+    int stem_stride, int max_num_q_blocks, int64_t ldQS, int64_t ldQS1, int64_t ldQS2,
+    cudaStream_t stream);
+/* block_logits [B, Hq, max_num_qb, max_num_kb] bf16 contiguous, every element written. No host
+ * synchronisation: capturable. */
+int hpc_stem_oam_gemm_dim128_async(
+    void* block_logits_ptr, const void* qflat_ptr, const void* kflat_ptr, const void* vbias_ptr,
+    const void* q_seq_lens_ptr, const void* kv_seq_lens_ptr, int num_batch, int num_head_q,
+    int num_head_kv, int max_num_qb, int max_num_kb, int stem_block_size, int stem_stride,
+    int causal, cudaStream_t stream);
+/* mask [B, Hq, max_Qb, max_Kb] u8, every byte written; max_Kb <= 32768. Capturable. */
+int hpc_stem_tpd_async(
+    void* mask_ptr, const void* block_logits_ptr, const void* q_seq_lens_ptr,
+    const void* kv_seq_lens_ptr, const void* num_prompt_tokens_ptr, int num_batch, int num_heads,
+    int max_Qb, int max_Kb, int block_size, float alpha, int initial_blocks, int window_size,
+    float k_block_num_rate_medium, int k_block_num_bias_medium, float k_block_num_rate_large,
+    int k_block_num_bias_large, cudaStream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

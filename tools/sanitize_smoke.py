@@ -1,5 +1,6 @@
 """One small invocation of every hot-path op (decode both quant types, prefill both, bf16 prefill
-dense and paged, blockwise + per-tensor MoE, route GEMM, W=1 allreduce, rope), meant to run under compute-sanitizer:
+dense and paged, blockwise + per-tensor MoE, route GEMM, W=1 allreduce, rope, the Stem mask stages),
+meant to run under compute-sanitizer:
 
     compute-sanitizer --tool memcheck  python tools/sanitize_smoke.py
     compute-sanitizer --tool synccheck python tools/sanitize_smoke.py
@@ -26,7 +27,7 @@ def cuda(d):
 
 def main():
     which = set(sys.argv[1:]) or {"decode", "prefill", "prefill_bf16", "moe", "gemm", "allreduce",
-                                  "rope"}
+                                  "rope", "stem"}
     if "decode" in which:
         B, hkv, hq = 3, 2, 8
         lens = [300, 129, 64]
@@ -112,6 +113,34 @@ def main():
                                      d["kv_indices"], d["q_norm_w"], d["k_norm_w"], 2)
         assert torch.allclose(q.float().cpu(), ref.float(), atol=8e-2) and torch.equal(c["vcache"].cpu(), vc)
         print("rope ok")
+    if "stem" in which:
+        import numpy as np
+        from oracle import stem as ost
+        from synth import stem as sst
+        for quant, page, layout in ((1, 64, "nhd"), (0, 32, "hnd")):
+            d = sst.make_inputs([300, 77, 0], [1100, 3000, 200], 4, 2, page, layout, quant, seed=9)
+            c = cuda(d)
+            kflat, vbias = hpc.stem_oam_prep_paged_kv(c["kcache"], c["vcache"], c["kscale"], c["vscale"],
+                                                      c["kv_indices"], c["kv_seq_lens"], 0.3,
+                                                      quant_type=hpc.QuantType(quant))
+            qflat = hpc.stem_oam_prep_varlen_q(c["q"], c["qscale"], c["q_seq_lens"], c["cu_seqlens_q"])
+            lg = hpc.stem_oam_gemm(qflat, kflat, vbias, c["q_seq_lens"], c["kv_seq_lens"])
+            mask = hpc.stem_tpd(lg, c["q_seq_lens"], c["kv_seq_lens"], c["kv_seq_lens"], alpha=0.5)
+            kv = ost.kv_prep(d["kcache"], d["vcache"], d["kscale"], d["vscale"], d["kv_indices"],
+                             d["kv_seq_lens"], 0.3, quant)
+            for b, o in enumerate(kv):
+                nkb = o["vbias"].shape[1]
+                assert (np.abs(kflat[b, :, :nkb].double().cpu().numpy() - o["kflat"]) <= o["kflat_bound"]).all()
+            y, bound, dead = ost.gemm(qflat.cpu(), kflat.cpu(), vbias.cpu(), d["q_seq_lens"], d["kv_seq_lens"])
+            lgc = lg.double().cpu().numpy()
+            assert np.array_equal(np.isneginf(lgc), dead) and (np.abs(lgc - y)[~dead] <= bound[~dead]).all()
+            want = ost.tpd(lg, d["q_seq_lens"], d["kv_seq_lens"], d["kv_seq_lens"], alpha=0.5)
+            assert np.array_equal(mask.cpu().numpy(), want)
+        wide = sst.adversarial_logits(1, 2, 3, 1500, seed=1)
+        ql, kl = torch.tensor([300], dtype=torch.int32), torch.tensor([1500 * 128], dtype=torch.int32)
+        m = hpc.stem_tpd(wide.cuda(), ql.cuda(), kl.cuda(), kl.cuda())
+        assert np.array_equal(m.cpu().numpy(), ost.tpd(wide, ql, kl, kl))
+        print("stem ok")
     torch.cuda.synchronize()
     print("smoke ok")
 
