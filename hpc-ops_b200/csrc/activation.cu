@@ -6,6 +6,10 @@
 //                       fused MoE pipeline this work is the epilogue of the Gate-Up GEMM instead)
 //   scaled_fp8_quant  : out[i] = e4m3( in[i] * (1 / scale) )                          in f32 / f16 / bf16
 //                       (reference src/activation/activation.cu:461-500, launcher :783-804)
+//   masked_act_mul_and_quant / masked_act_mul_and_blockwise_quant : the same silu(gate) * up over
+//                       the per-expert padded (DeepEP low-latency) layout [E * T_max, 2C], valid rows
+//                       only, per-tensor or 1x128 blockwise e4m3 (reference activation.cu:203-280 and
+//                       :358-433; there every thread visits every padded row)
 //   gather_rows       : dst[i, :] = src[row_indices[i], :]   (the A-operand gather of the reference's
 //                       scatter grouped GEMM, src/group_gemm/cp_async/group_gemm_fp8_scatter.cu:20-46,
 //                       done here as a streaming pre-pass in front of the TMA-fed grouped GEMM)
@@ -23,6 +27,40 @@ constexpr int kThreads = 256;
 
 __device__ __forceinline__ float silu_exact(float x) { return x / (1.f + expf(-x)); }
 
+// silu(gate) * up for the 8 columns at `g` (gate) and `g + half_col` (up) of one row: 16 B of
+// gate + 16 B of up in. With `use_bf16_mul` the product is formed in bf16 as the reference kernel
+// and its test do; otherwise in fp32.
+__device__ __forceinline__ void silu_mul8(const __nv_bfloat16* g, int half_col, int use_bf16_mul,
+                                          float (&m)[8]) {
+  const uint4 gv = ld_nc_v4(g);
+  const uint4 uv = ld_nc_v4(g + half_col);
+  const __nv_bfloat162* g2 = reinterpret_cast<const __nv_bfloat162*>(&gv);
+  const __nv_bfloat162* u2 = reinterpret_cast<const __nv_bfloat162*>(&uv);
+#pragma unroll
+  for (int i = 0; i < 4; i++) {
+    const float2 gf = __bfloat1622float2(g2[i]);
+    const float s0 = silu_exact(gf.x), s1 = silu_exact(gf.y);
+    if (use_bf16_mul) {
+      const __nv_bfloat162 p = __hmul2(__floats2bfloat162_rn(s0, s1), u2[i]);
+      const float2 pf = __bfloat1622float2(p);
+      m[2 * i] = pf.x;
+      m[2 * i + 1] = pf.y;
+    } else {
+      const float2 uf = __bfloat1622float2(u2[i]);
+      m[2 * i] = s0 * uf.x;
+      m[2 * i + 1] = s1 * uf.y;
+    }
+  }
+}
+
+// 8 values times `scale` -> 8 e4m3 bytes
+__device__ __forceinline__ uint2 quant8(const float (&m)[8], float scale) {
+  uint2 w;
+  w.x = cvt_e4m3x4(m[0] * scale, m[1] * scale, m[2] * scale, m[3] * scale);
+  w.y = cvt_e4m3x4(m[4] * scale, m[5] * scale, m[6] * scale, m[7] * scale);
+  return w;
+}
+
 // one thread = 8 output columns of one row: 16 B of gate + 16 B of up in, 8 B out
 __global__ void __launch_bounds__(kThreads)
     act_mul_and_quant_kernel(uint8_t* __restrict__ out, const __nv_bfloat16* __restrict__ in,
@@ -35,32 +73,103 @@ __global__ void __launch_bounds__(kThreads)
        v += static_cast<long long>(gridDim.x) * kThreads) {
     const long long r = v / vec_per_row;
     const int c = static_cast<int>(v - r * vec_per_row) << 3;
-    const __nv_bfloat16* g = in + r * (2LL * half_col) + c;
-    const uint4 gv = ld_nc_v4(g);
-    const uint4 uv = ld_nc_v4(g + half_col);
-    const __nv_bfloat162* g2 = reinterpret_cast<const __nv_bfloat162*>(&gv);
-    const __nv_bfloat162* u2 = reinterpret_cast<const __nv_bfloat162*>(&uv);
     float m[8];
+    silu_mul8(in + r * (2LL * half_col) + c, half_col, use_bf16_mul, m);
+    *reinterpret_cast<uint2*>(out + r * half_col + c) = quant8(m, scale);
+  }
+}
+
+// ---- masked (per-expert padded) layout ---------------------------------------------------------
+// Row e * T_max + t of [E * T_max, 2C] is valid when t < clamp(num_per_expert[e], 0, T_max). Each
+// CTA reads the E counts once into an exclusive prefix sum in shared memory (warp 0, 32 experts per
+// step), then strides over the (valid row, 8 columns) items only: item i is the (i / vpr)-th valid
+// row, whose expert is found by binary search in the prefix. Invalid rows are neither read nor
+// written, and the work follows the number of valid rows, not E * T_max.
+__device__ __forceinline__ void expert_prefix(const int* __restrict__ num_per_expert, int num_expert,
+                                              int t_max, int* prefix) {
+  if (threadIdx.x < 32) {
+    const int lane = threadIdx.x;
+    int carry = 0;
+    if (lane == 0) prefix[0] = 0;
+    for (int base = 0; base < num_expert; base += 32) {
+      int c = base + lane < num_expert ? __ldg(num_per_expert + base + lane) : 0;
+      c = min(max(c, 0), t_max);
 #pragma unroll
-    for (int i = 0; i < 4; i++) {
-      const float2 gf = __bfloat1622float2(g2[i]);
-      const float s0 = silu_exact(gf.x), s1 = silu_exact(gf.y);
-      if (use_bf16_mul) {
-        // bf16(silu(gate)) * up with a bf16-rounded product, as the reference kernel and its test do
-        const __nv_bfloat162 p = __hmul2(__floats2bfloat162_rn(s0, s1), u2[i]);
-        const float2 pf = __bfloat1622float2(p);
-        m[2 * i] = pf.x;
-        m[2 * i + 1] = pf.y;
-      } else {
-        const float2 uf = __bfloat1622float2(u2[i]);
-        m[2 * i] = s0 * uf.x;
-        m[2 * i + 1] = s1 * uf.y;
+      for (int o = 1; o < 32; o <<= 1) {
+        const int n = __shfl_up_sync(0xffffffffu, c, o);
+        if (lane >= o) c += n;
       }
+      if (base + lane < num_expert) prefix[base + lane + 1] = carry + c;
+      carry += __shfl_sync(0xffffffffu, c, 31);
     }
-    uint2 w;
-    w.x = cvt_e4m3x4(m[0] * scale, m[1] * scale, m[2] * scale, m[3] * scale);
-    w.y = cvt_e4m3x4(m[4] * scale, m[5] * scale, m[6] * scale, m[7] * scale);
-    *reinterpret_cast<uint2*>(out + r * half_col + c) = w;
+  }
+  __syncthreads();
+}
+
+// the padded row of the k-th valid row: the expert e with prefix[e] <= k < prefix[e + 1]
+__device__ __forceinline__ long long valid_row(const int* prefix, int num_expert, int t_max, int k) {
+  int lo = 0, hi = num_expert;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (prefix[mid + 1] <= k) lo = mid + 1;
+    else hi = mid;
+  }
+  return static_cast<long long>(lo) * t_max + (k - prefix[lo]);
+}
+
+// per-tensor: out = e4m3(silu(gate) * up * scale[0]), the row body of act_mul_and_quant
+// (use_bf16_mul = 0)
+__global__ void __launch_bounds__(kThreads)
+    masked_act_mul_and_quant_kernel(uint8_t* __restrict__ out, const __nv_bfloat16* __restrict__ in,
+                                    const float* __restrict__ scale_ptr,
+                                    const int* __restrict__ num_per_expert, int num_expert,
+                                    int t_max, int half_col) {
+  extern __shared__ int prefix[];
+  expert_prefix(num_per_expert, num_expert, t_max, prefix);
+  const float scale = __ldg(scale_ptr);
+  const int vpr = half_col >> 3;
+  const int total = prefix[num_expert] * vpr;  // < 2^31, checked by the launcher
+  for (int v = blockIdx.x * kThreads + threadIdx.x; v < total; v += gridDim.x * kThreads) {
+    const int k = v / vpr;
+    const int c = (v - k * vpr) << 3;
+    const long long r = valid_row(prefix, num_expert, t_max, k);
+    float m[8];
+    silu_mul8(in + r * (2LL * half_col) + c, half_col, 0, m);
+    *reinterpret_cast<uint2*>(out + r * half_col + c) = quant8(m, scale);
+  }
+}
+
+// blockwise: per (row, 128 columns) = 16 lanes x 8 columns, sc = amax / 448,
+// out = e4m3(v * (1 / (sc + 1e-8))), out_scale[row, block] = sc (row-major [E * T_max, C / 128]).
+// vpr is a multiple of 16 and so is every item index a half-warp starts at, so the 16 lanes of a
+// 128-column block are always the 16 lanes of one half-warp and reach the loop test together.
+__global__ void __launch_bounds__(kThreads)
+    masked_act_mul_and_blockwise_quant_kernel(uint8_t* __restrict__ out,
+                                              float* __restrict__ out_scale,
+                                              const __nv_bfloat16* __restrict__ in,
+                                              const int* __restrict__ num_per_expert,
+                                              int num_expert, int t_max, int half_col) {
+  extern __shared__ int prefix[];
+  expert_prefix(num_per_expert, num_expert, t_max, prefix);
+  const int vpr = half_col >> 3;
+  const int total = prefix[num_expert] * vpr;
+  const int lane = threadIdx.x & 31;
+  const unsigned half_mask = 0xffffu << (lane & 16);
+  for (int v = blockIdx.x * kThreads + threadIdx.x; v < total; v += gridDim.x * kThreads) {
+    const int k = v / vpr;
+    const int c = (v - k * vpr) << 3;
+    const long long r = valid_row(prefix, num_expert, t_max, k);
+    float m[8];
+    silu_mul8(in + r * (2LL * half_col) + c, half_col, 0, m);
+    float amax = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; i++) amax = fmaxf(amax, fabsf(m[i]));
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(half_mask, amax, o));
+    const float sc = amax / 448.0f;
+    const float inv = 1.0f / (sc + 1e-8f);
+    *reinterpret_cast<uint2*>(out + r * half_col + c) = quant8(m, inv);
+    if ((lane & 15) == 0) out_scale[r * (half_col >> 7) + (c >> 7)] = sc;
   }
 }
 
@@ -154,6 +263,82 @@ extern "C" int hpc_act_mul_and_quant_async(void* y_ptr, const void* x_ptr, const
   act::act_mul_and_quant_kernel<<<act::stream_grid(items), act::kThreads, 0, stream>>>(
       static_cast<uint8_t*>(y_ptr), static_cast<const __nv_bfloat16*>(x_ptr), scale_ptr, num_row,
       half, use_bf16_mul);
+  HPC_CUDA_CHECK(cudaGetLastError());
+  return HPC_OK;
+}
+
+// Shared argument checks of the two masked launchers; sets *items and *smem.
+static int masked_setup(const char* what, const void* y_ptr, const void* x_ptr,
+                        const void* num_per_expert_ptr, int num_total_tokens,
+                        int num_intermediate_size, int num_tokens_per_expert, int col_multiple,
+                        int* items_out, size_t* smem) {
+  HPC_REQUIRE(num_intermediate_size > 0 && num_intermediate_size % col_multiple == 0,
+              "%s: intermediate size (%d) must be a positive multiple of %d", what,
+              num_intermediate_size, col_multiple);
+  HPC_REQUIRE(num_tokens_per_expert > 0 && num_total_tokens >= 0 &&
+                  num_total_tokens % num_tokens_per_expert == 0,
+              "%s: rows (%d) must be a multiple of the tokens per expert (%d)", what,
+              num_total_tokens, num_tokens_per_expert);
+  const int num_expert = num_total_tokens / num_tokens_per_expert;
+  HPC_REQUIRE(num_expert <= 8192, "%s: %d experts exceed the supported 8192", what, num_expert);
+  HPC_REQUIRE(num_expert == 0 || num_per_expert_ptr != nullptr, "%s: num_per_expert missing", what);
+  HPC_REQUIRE((reinterpret_cast<uintptr_t>(x_ptr) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(y_ptr) & 7) == 0,
+              "%s: input must be 16-byte and output 8-byte aligned", what);
+  // the kernels index items in 32 bits: items plus one grid stride (<= 8 * 256 per SM) must fit
+  const long long items = static_cast<long long>(num_total_tokens) * (num_intermediate_size / 8);
+  HPC_REQUIRE(items <= (1LL << 30), "%s: %lld 8-column items exceed the supported 2^30", what,
+              items);
+  *items_out = static_cast<int>(items);
+  *smem = static_cast<size_t>(num_expert + 1) * sizeof(int);
+  return HPC_OK;
+}
+
+// replaces reference src/activation/activation.h (masked_act_mul_and_quant_async).
+// input bf16 [num_total_tokens, 2 * num_intermediate_size], rows grouped per expert in blocks of
+// num_tokens_per_expert; only the first clamp(num_per_expert[e], 0, T_max) rows of expert e are
+// read and written.
+extern "C" int hpc_masked_act_mul_and_quant_async(void* output_ptr, const void* input_ptr,
+                                                  const float* scale_ptr,
+                                                  const int* num_per_expert_ptr,
+                                                  int num_total_tokens, int num_intermediate_size,
+                                                  int num_tokens_per_expert, cudaStream_t stream) {
+  int items = 0;
+  size_t smem = 0;
+  const int rc = masked_setup("masked_act_mul_and_quant", output_ptr, input_ptr, num_per_expert_ptr,
+                              num_total_tokens, num_intermediate_size, num_tokens_per_expert, 8,
+                              &items, &smem);
+  if (rc != HPC_OK) return rc;
+  if (num_total_tokens == 0) return HPC_OK;
+  const int grid = act::stream_grid(items);
+  act::masked_act_mul_and_quant_kernel<<<grid, act::kThreads, smem, stream>>>(
+      static_cast<uint8_t*>(output_ptr), static_cast<const __nv_bfloat16*>(input_ptr), scale_ptr,
+      num_per_expert_ptr, num_total_tokens / num_tokens_per_expert, num_tokens_per_expert,
+      num_intermediate_size);
+  HPC_CUDA_CHECK(cudaGetLastError());
+  return HPC_OK;
+}
+
+// replaces reference src/activation/activation.h (masked_act_mul_and_blockwise_quant_async).
+// output_scale f32 row-major [num_total_tokens, num_intermediate_size / 128].
+extern "C" int hpc_masked_act_mul_and_blockwise_quant_async(
+    void* output_ptr, float* output_scale_ptr, const void* input_ptr, const int* num_per_expert_ptr,
+    int num_total_tokens, int num_intermediate_size, int num_tokens_per_expert,
+    cudaStream_t stream) {
+  int items = 0;
+  size_t smem = 0;
+  const int rc = masked_setup("masked_act_mul_and_blockwise_quant", output_ptr, input_ptr,
+                              num_per_expert_ptr, num_total_tokens, num_intermediate_size,
+                              num_tokens_per_expert, 128, &items, &smem);
+  if (rc != HPC_OK) return rc;
+  HPC_REQUIRE((reinterpret_cast<uintptr_t>(output_scale_ptr) & 3) == 0,
+              "masked_act_mul_and_blockwise_quant: output_scale must be 4-byte aligned");
+  if (num_total_tokens == 0) return HPC_OK;
+  const int grid = act::stream_grid(items);
+  act::masked_act_mul_and_blockwise_quant_kernel<<<grid, act::kThreads, smem, stream>>>(
+      static_cast<uint8_t*>(output_ptr), output_scale_ptr,
+      static_cast<const __nv_bfloat16*>(input_ptr), num_per_expert_ptr,
+      num_total_tokens / num_tokens_per_expert, num_tokens_per_expert, num_intermediate_size);
   HPC_CUDA_CHECK(cudaGetLastError());
   return HPC_OK;
 }

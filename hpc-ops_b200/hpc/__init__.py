@@ -12,7 +12,7 @@ from . import _ops as _ops_mod
 
 # in-scope modules of the reference package, in import order
 _MODULES = ("attention", "group_gemm", "fuse_moe", "act", "gemm", "multicast_handle", "communicator",
-            "allreduce", "rope", "sampler", "stem")
+            "allreduce", "rope", "sampler", "stem", "normalization")
 
 __all__ = []
 for _name in _MODULES:

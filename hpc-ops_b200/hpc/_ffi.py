@@ -100,7 +100,8 @@ lib.hpc_attention_blocksparse_prefill_qkpertoken_perhead_vperhead_fp8_async.argt
     _prefill_args + [c_i64] * 3 + [c_ptr])
 
 # (hasattr: a library built from an older commit, e.g. for an A/B timing, lacks these symbols; it
-# still fails loudly -- at the first rope, sampler or bf16 prefill call)
+# still fails loudly -- at the first rope, sampler, bf16 prefill, Stem, RMSNorm or masked
+# activation call)
 if hasattr(lib, "hpc_rope_norm_store_kv_async"):
     lib.hpc_rope_norm_store_kv_async.restype = c_int
     lib.hpc_rope_norm_store_kv_async.argtypes = [c_ptr] * 12 + [c_int] * 12 + [c_ptr]
@@ -141,6 +142,14 @@ if hasattr(lib, "hpc_stem_tpd_async"):
     lib.hpc_stem_tpd_async.argtypes = (
         [c_ptr] * 5 + [c_int] * 5 + [c_f32, c_int, c_int, c_f32, c_int, c_f32, c_int, c_ptr])
 
+
+if hasattr(lib, "hpc_fused_rmsnorm_with_scale_async"):
+    lib.hpc_fused_rmsnorm_with_scale_async.restype = c_int
+    lib.hpc_fused_rmsnorm_with_scale_async.argtypes = [c_ptr] * 6 + [c_f32] + [c_int] * 3 + [c_ptr]
+    lib.hpc_masked_act_mul_and_quant_async.restype = c_int
+    lib.hpc_masked_act_mul_and_quant_async.argtypes = [c_ptr] * 4 + [c_int] * 3 + [c_ptr]
+    lib.hpc_masked_act_mul_and_blockwise_quant_async.restype = c_int
+    lib.hpc_masked_act_mul_and_blockwise_quant_async.argtypes = [c_ptr] * 4 + [c_int] * 3 + [c_ptr]
 
 def check(rc: int, what: str = ""):
     """Turn a launcher status into the RuntimeError the reference raises via TORCH_CHECK."""

@@ -1,5 +1,6 @@
-"""Stand-alone activation / FP8 quantisation operators (API of reference hpc/act.py; the masked
-DeepEP-layout variants are out of scope, SURVEY.md §2 row 6)."""
+"""Stand-alone activation / FP8 quantisation operators (API of reference hpc/act.py), including the
+masked variants over the per-expert padded (DeepEP low-latency) layout [E * T_max, 2C], which read
+and write only each expert's first num_per_expert[e] rows."""
 from typing import Optional, Tuple
 
 import torch
@@ -61,11 +62,71 @@ def _scaled_fp8_quant_impl(input, scale, output):
     return output, scale
 
 
+def _masked_args(what, input, num_per_expert, col_multiple):
+    # reference src/activation/entry.cc:52-156, plus the layout checks it leaves out
+    _require(input.is_cuda and num_per_expert.is_cuda and num_per_expert.device == input.device,
+             f"{what}: input and num_per_expert must be on the same CUDA device")
+    _require(input.dtype == torch.bfloat16 and input.dim() == 2 and input.is_contiguous(),
+             f"{what}: input must be a contiguous bfloat16 [N, 2C] tensor")
+    _require(num_per_expert.dtype == torch.int32 and num_per_expert.dim() == 1
+             and num_per_expert.is_contiguous() and num_per_expert.numel() >= 1,
+             f"{what}: num_per_expert must be a contiguous int32 [E] tensor")
+    n, two_c = input.shape
+    c = two_c // 2
+    _require(two_c % 2 == 0 and c > 0 and c % col_multiple == 0,
+             f"{what}: intermediate size {c} must be a positive multiple of {col_multiple}")
+    e = num_per_expert.numel()
+    _require(n % e == 0, f"{what}: rows ({n}) must be a multiple of the number of experts ({e})")
+    return n, c, n // e
+
+
+def _check_out(what, name, t, shape, dtype, device):
+    _require(t.dtype == dtype and tuple(t.shape) == tuple(shape) and t.device == device
+             and t.is_contiguous(),
+             f"{what}: {name} must be a contiguous {dtype} tensor of shape {list(shape)} on "
+             f"{device}, got {t.dtype} {list(t.shape)} on {t.device}")
+
+
+def _masked_act_mul_and_quant_impl(input, scale, num_per_expert, output):
+    what = "masked_act_mul_and_quant"
+    n, c, t_max = _masked_args(what, input, num_per_expert, 8)
+    _require(scale.is_cuda and scale.device == input.device and scale.dtype == torch.float32
+             and scale.numel() == 1, f"{what}: scale must be one float32 value on the input's device")
+    if output is None:
+        output = torch.empty((n, c), dtype=torch.float8_e4m3fn, device=input.device)
+    _check_out(what, "output", output, (n, c), torch.float8_e4m3fn, input.device)
+    _check_rc(_lib.hpc_masked_act_mul_and_quant_async(
+        _ptr(output), _ptr(input), _ptr(scale), _ptr(num_per_expert), n, c, t_max,
+        _stream_of(input)), what)
+    return output
+
+
+def _masked_act_mul_and_blockwise_quant_impl(input, num_per_expert, output, output_scale):
+    what = "masked_act_mul_and_blockwise_quant"
+    n, c, t_max = _masked_args(what, input, num_per_expert, 128)
+    if output is None:
+        output = torch.empty((n, c), dtype=torch.float8_e4m3fn, device=input.device)
+    if output_scale is None:
+        output_scale = torch.empty((n, c // 128), dtype=torch.float32, device=input.device)
+    _check_out(what, "output", output, (n, c), torch.float8_e4m3fn, input.device)
+    _check_out(what, "output_scale", output_scale, (n, c // 128), torch.float32, input.device)
+    _check_rc(_lib.hpc_masked_act_mul_and_blockwise_quant_async(
+        _ptr(output), _ptr(output_scale), _ptr(input), _ptr(num_per_expert), n, c, t_max,
+        _stream_of(input)), what)
+    return output, output_scale
+
+
 _ops.define("act_mul_and_quant(Tensor input, Tensor scale, bool use_bf16_mul, Tensor? output) -> "
             "(Tensor)")
 _ops.impl("act_mul_and_quant", _act_mul_and_quant_impl, "CUDA")
 _ops.define("scaled_fp8_quant(Tensor input, Tensor? scale, Tensor? output) -> (Tensor, Tensor)")
 _ops.impl("scaled_fp8_quant", _scaled_fp8_quant_impl, "CUDA")
+_ops.define("masked_act_mul_and_quant(Tensor input, Tensor scale, Tensor num_per_expert, "
+            "Tensor? output) -> (Tensor)")
+_ops.impl("masked_act_mul_and_quant", _masked_act_mul_and_quant_impl, "CUDA")
+_ops.define("masked_act_mul_and_blockwise_quant(Tensor input, Tensor num_per_expert, Tensor? output, "
+            "Tensor? output_scale) -> (Tensor output, Tensor output_scale)")
+_ops.impl("masked_act_mul_and_blockwise_quant", _masked_act_mul_and_blockwise_quant_impl, "CUDA")
 
 
 def act_mul_and_quant(gate_up: Tensor, scale: Tensor, use_bf16_mul: bool = True,
@@ -83,6 +144,28 @@ def scaled_fp8_quant(input: Tensor, scale: Optional[Tensor] = None,
     return torch.ops.hpc.scaled_fp8_quant(input, scale, output)
 
 
+def masked_act_mul_and_quant(gate_up: Tensor, scale: Tensor, num_per_expert: Tensor,
+                             output: Optional[Tensor] = None) -> Tensor:
+    """silu(gate) * up * scale[0] -> fp8_e4m3 [N, C] over the per-expert padded layout
+    gate_up bf16 [N = E * T_max, 2C] (C % 8 == 0), computed in fp32 as act_mul_and_quant with
+    use_bf16_mul=False. Row e * T_max + t is valid when t < clamp(num_per_expert[e], 0, T_max)
+    (num_per_expert int32 [E] on the device); only valid rows are read and written, so the other
+    rows of a provided `output` keep their contents (reference hpc/act.py:37-67)."""
+    return torch.ops.hpc.masked_act_mul_and_quant(gate_up, scale, num_per_expert, output)
+
+
+def masked_act_mul_and_blockwise_quant(gate_up: Tensor, num_per_expert: Tensor,
+                                       output: Optional[Tensor] = None,
+                                       output_scale: Optional[Tensor] = None
+                                       ) -> Tuple[Tensor, Tensor]:
+    """The masked layout of masked_act_mul_and_quant with 1x128 blockwise quantisation
+    (C % 128 == 0): per (row, 128 columns) of v = silu(gate) * up, sc = amax|v| / 448 and
+    out = e4m3(v / (sc + 1e-8)); returns (out [N, C], sc f32 row-major [N, C / 128]). Invalid rows
+    of provided outputs keep their contents (reference hpc/act.py:70-105)."""
+    return torch.ops.hpc.masked_act_mul_and_blockwise_quant(gate_up, num_per_expert, output,
+                                                            output_scale)
+
+
 @torch.library.register_fake("hpc::act_mul_and_quant")
 def _act_mul_and_quant_fake(input, scale, use_bf16_mul, output):
     shape = list(input.shape)
@@ -93,3 +176,16 @@ def _act_mul_and_quant_fake(input, scale, use_bf16_mul, output):
 @torch.library.register_fake("hpc::scaled_fp8_quant")
 def _scaled_fp8_quant_fake(input, scale, output):
     return torch.empty_like(input, dtype=torch.float8_e4m3fn), scale
+
+
+@torch.library.register_fake("hpc::masked_act_mul_and_quant")
+def _masked_act_mul_and_quant_fake(input, scale, num_per_expert, output):
+    return torch.empty(input.shape[0], input.shape[1] // 2, dtype=torch.float8_e4m3fn,
+                       device=input.device)
+
+
+@torch.library.register_fake("hpc::masked_act_mul_and_blockwise_quant")
+def _masked_act_mul_and_blockwise_quant_fake(input, num_per_expert, output, output_scale):
+    n, c = input.shape[0], input.shape[1] // 2
+    return (torch.empty(n, c, dtype=torch.float8_e4m3fn, device=input.device),
+            torch.empty(n, c // 128, dtype=torch.float32, device=input.device))

@@ -171,6 +171,34 @@ int hpc_act_mul_and_quant_async(void* y_ptr, const void* x_ptr, const float* sca
                                 int num_col, int use_bf16_mul, cudaStream_t stream);
 int hpc_scaled_fp8_quant_async(void* y_ptr, const void* x_ptr, const float* scale_ptr,
                                int64_t numel, int in_dtype, cudaStream_t stream);
+/* Masked (per-expert padded, DeepEP low-latency) layout: input bf16 [N = E * T_max, 2C], rows
+ * e * T_max + t with t < clamp(num_per_expert[e], 0, T_max) valid (num_per_expert int32 [E] on the
+ * device), N % T_max == 0, 16-byte aligned input. Only valid rows of the outputs are written; the
+ * others keep whatever the caller's buffer held. Per-tensor: e4m3(silu(gate) * up * scale[0]) in
+ * fp32 (act_mul_and_quant with use_bf16_mul = 0), C % 8 == 0. Blockwise: per (row, 128 columns)
+ * sc = amax / 448, out = e4m3(v / (sc + 1e-8)), output_scale f32 row-major [N, C / 128],
+ * C % 128 == 0. Stream-ordered, no allocation or host synchronisation: capturable. */
+int hpc_masked_act_mul_and_quant_async(void* output_ptr, const void* input_ptr,
+                                       const float* scale_ptr, const int* num_per_expert_ptr,
+                                       int num_total_tokens, int num_intermediate_size,
+                                       int num_tokens_per_expert, cudaStream_t stream);
+int hpc_masked_act_mul_and_blockwise_quant_async(void* output_ptr, float* output_scale_ptr,
+                                                 const void* input_ptr,
+                                                 const int* num_per_expert_ptr,
+                                                 int num_total_tokens, int num_intermediate_size,
+                                                 int num_tokens_per_expert, cudaStream_t stream);
+
+/* ---- fused RMSNorm -> FP8 --------------------------------------------------------------------------
+ * replaces reference src/normalization/fused_rmsnorm_with_scale.h. input bf16 [batch_size,
+ * hidden_state] (rows contiguous), weight bf16 [hidden_state], scale f32 on the device ([1], or [2]
+ * with is_moe). y = (x * w) * rsqrtf(sum(x^2) / H + eps) in fp32; output = e4m3_rn_satfinite(
+ * y * (1 / scale[0])); with is_moe also output_fp32 = y and output_fp8_scale2 =
+ * e4m3_rn_satfinite(y * (1 / scale[1])). Any hidden_state % 8 == 0 in [8, 16384]. Capturable. */
+int hpc_fused_rmsnorm_with_scale_async(const void* input_ptr, const void* weight_ptr,
+                                       void* output_ptr, void* output_fp32_ptr,
+                                       void* output_fp8_scale2_ptr, const void* scale_ptr,
+                                       float eps, int batch_size, int hidden_state, int is_moe,
+                                       cudaStream_t stream);
 
 /* ---- FusedMoE -----------------------------------------------------------------------------------
  * replace reference src/fuse_moe/fuse_moe.h:15-62, argument for argument (bool -> int).

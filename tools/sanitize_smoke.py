@@ -1,5 +1,6 @@
 """One small invocation of every hot-path op (decode both quant types, prefill both, bf16 prefill
-dense and paged, blockwise + per-tensor MoE, route GEMM, W=1 allreduce, rope, the Stem mask stages),
+dense and paged, blockwise + per-tensor MoE, route GEMM, W=1 allreduce, rope, the Stem mask stages,
+fused RMSNorm -> FP8 and the masked activation quantisers),
 meant to run under compute-sanitizer:
 
     compute-sanitizer --tool memcheck  python tools/sanitize_smoke.py
@@ -27,7 +28,7 @@ def cuda(d):
 
 def main():
     which = set(sys.argv[1:]) or {"decode", "prefill", "prefill_bf16", "moe", "gemm", "allreduce",
-                                  "rope", "stem"}
+                                  "rope", "stem", "norm_act"}
     if "decode" in which:
         B, hkv, hq = 3, 2, 8
         lens = [300, 129, 64]
@@ -141,6 +142,25 @@ def main():
         m = hpc.stem_tpd(wide.cuda(), ql.cuda(), kl.cuda(), kl.cuda())
         assert np.array_equal(m.cpu().numpy(), ost.tpd(wide, ql, kl, kl))
         print("stem ok")
+    if "norm_act" in which:
+        from oracle import masked_act as oact, normalization as onorm
+        from synth import act as sact, normalization as snorm
+        d = snorm.make_inputs(5, 1032, seed=11, device="cuda")
+        out = hpc.fused_rmsnorm_with_scale(d["x"], d["w"], d["eps"], d["scale"], True)
+        res = onorm.check(out, d["x"], d["w"], d["eps"], d["scale"], True)
+        assert not onorm.failed(res), res
+        for blockwise in (False, True):
+            d = sact.make_inputs(6, 5, 256, seed=12, device="cuda")
+            sent = sact.sentinel_outputs(30, 256, device="cuda")
+            o, s = sent[0].clone(), sent[1].clone()
+            if blockwise:
+                hpc.masked_act_mul_and_blockwise_quant(d["gate_up"], d["num_per_expert"], o, s)
+            else:
+                hpc.masked_act_mul_and_quant(d["gate_up"], d["scale"], d["num_per_expert"], o)
+            res = oact.masked_check(o, s if blockwise else None, d["gate_up"], d["num_per_expert"], 5,
+                                    sent, scale=d["scale"])
+            assert oact.masked_ok(res), res
+        print("norm_act ok")
     torch.cuda.synchronize()
     print("smoke ok")
 
