@@ -19,21 +19,7 @@ sys.path.insert(0, str(REPO / "hpc-ops_b200"))
 import torch  # noqa: E402
 import torch.distributed as dist  # noqa: E402
 
-
-def timed(fn, iters, warm=5):
-    for _ in range(warm):
-        fn()
-    dist.barrier()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    t = torch.tensor([e0.elapsed_time(e1) / iters], device="cuda", dtype=torch.float64)
-    dist.all_reduce(t, op=dist.ReduceOp.MAX)
-    return float(t.item())
+from timing import NVLINK_GBS, card, time_eager  # noqa: E402
 
 
 def _rmsnorm(x, w, eps):
@@ -79,6 +65,9 @@ def main():
     comm.Barrier()
     nbytes = n_pad * H * 2
     results = []
+    gpu = card()
+    if rank == 0:
+        print(json.dumps({"card": gpu}), flush=True)
 
     def emit(d):
         d.update(world=world, tokens=T, hidden=H, multicast=bool(in_hdl.has_multicast))
@@ -101,11 +90,11 @@ def main():
         torch.cuda.synchronize()
         comm.Barrier()
         err = (out_x[s:e].float() - ref_out[s:e].float()).abs().max().item()  # own slice: residual is per rank
-        ms = timed(ht, a.iters)
+        ms = time_eager(ht, a.iters, warm=5, dist=dist)
         algbw = nbytes / ms / 1e6
         emit(dict(path="HT", blocks=blocks, ms=ms, algbw_gbs=algbw,
                   busbw_gbs=algbw * 2 * (world - 1) / max(world, 1), max_abs_err=err,
-                  frac_nvlink_770=(algbw * 2 * (world - 1) / world / 770) if world > 1 else None,
+                  frac_nvlink_770=(algbw * 2 * (world - 1) / world / NVLINK_GBS) if world > 1 else None,
                   hbm_gbs_w1=(4 * nbytes / ms / 1e6) if world == 1 else None))
 
     # ---- NCCL all_reduce + torch RMSNorm (unfused baseline) ----
@@ -115,12 +104,12 @@ def main():
         dist.all_reduce(buf)
         r = buf + residual
         _rmsnorm(r, weight, 1e-6)
-    ms = timed(nccl, max(5, a.iters // 5))
+    ms = time_eager(nccl, max(5, a.iters // 5), warm=5, dist=dist)
     emit(dict(path="NCCL+torch", ms=ms, algbw_gbs=nbytes / ms / 1e6))
 
     def nccl_only():
         dist.all_reduce(buf)
-    ms = timed(nccl_only, max(5, a.iters // 5))
+    ms = time_eager(nccl_only, max(5, a.iters // 5), warm=5, dist=dist)
     emit(dict(path="NCCL allreduce only", ms=ms, algbw_gbs=nbytes / ms / 1e6,
               busbw_gbs=nbytes / ms / 1e6 * 2 * (world - 1) / max(world, 1)))
 
@@ -147,19 +136,19 @@ def main():
         ll()
         torch.cuda.synchronize()
         err = (o.float() - ref_out[:t_ll].float()).abs().max().item()
-        ms = timed(ll, a.iters)
+        ms = time_eager(ll, a.iters, warm=5, dist=dist)
         emit(dict(path="LL", ll_tokens=t_ll, us=ms * 1e3, max_abs_err=err))
         xb = xi.clone()
 
         def nccl_small():
             dist.all_reduce(xb)
-        ms2 = timed(nccl_small, a.iters)
+        ms2 = time_eager(nccl_small, a.iters, warm=5, dist=dist)
         emit(dict(path="NCCL allreduce only", ll_tokens=t_ll, us=ms2 * 1e3))
 
     if rank == 0:
         out = REPO / "gpurun_out" / f"allreduce_bench_w{world}.json"
         out.parent.mkdir(exist_ok=True)
-        out.write_text(json.dumps(results, indent=1))
+        out.write_text(json.dumps({"card": gpu, "rows": results}, indent=1))
     dist.destroy_process_group()
 
 

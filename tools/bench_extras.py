@@ -5,84 +5,15 @@ Every entry times the public `hpc.*` call with CUDA events (graph replay where t
 benchmark does so), reports the figure against the relevant roofline, and carries a SAMPLED parity
 check against the CPU oracle on the very tensors that were timed (`oracle/` is imported only inside
 the `_oracle_*` helpers — the checker legs, the same role as bench.py's cpu_baseline leg).
-GPU box only; imported by bench.py and by tools/*_bench.py.
+Needs a GPU; imported by bench.py, tools/moe_bench.py and tools/prefill_bench.py. Timers and
+peaks come from tools/timing.py.
 """
-import json
 import math
 import time
-from pathlib import Path
 
 import torch
 
-REPO = Path(__file__).resolve().parents[1]
-
-FP8_NOMINAL_TFLOPS = 1979.0  # dense e4m3, H100 SXM data sheet (700 W)
-NVLINK_GBS = 450.0           # NVLink 4 per direction, H100 SXM data sheet (not measured)
-
-
-def peaks():
-    f = REPO / "MEASURED_PEAKS.json"
-    d = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "source": "H100 SXM data sheet (not measured)"}
-    if f.exists():
-        try:
-            j = json.loads(f.read_text())
-            d = {"hbm_gbs": float(j["hbm_gbs"]), "bf16_tflops": float(j["bf16_tflops"]),
-                 "source": "measured (MEASURED_PEAKS.json)"}
-        except Exception:
-            pass
-    # no measured FP8 entry exists: 2x the measured cuBLAS bf16 burst is the practical tensor roof
-    d["fp8_tflops_2x_bf16"] = 2 * d["bf16_tflops"]
-    return d
-
-
-def time_eager(fn, iters, warm=3):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters
-
-
-def time_graph(fn, reps=20, iters=5, dist=None):
-    """ms per call: `reps` back-to-back calls captured in one CUDA graph, replayed `iters` times
-    (the reference harness times graph replays: benchmark/fuse_allreduce_rmsorm/...:116-170).
-    With `dist` the ranks start together and the maximum over ranks is returned."""
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(3):
-            fn()
-    torch.cuda.current_stream().wait_stream(s)
-    torch.cuda.synchronize()
-    if dist is not None:
-        dist.barrier()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        for _ in range(reps):
-            fn()
-    g.replay()
-    torch.cuda.synchronize()
-    if dist is not None:
-        dist.barrier()
-        torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        g.replay()
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / (iters * reps)
-    if dist is not None:
-        t = torch.tensor([ms], dtype=torch.float64, device="cuda")
-        dist.all_reduce(t, op=dist.ReduceOp.MAX)
-        ms = float(t.item())
-    del g
-    return ms
+from timing import FP8_TFLOPS, NVLINK_GBS, peaks, time_eager, time_graph
 
 
 def _err_stats(my, gt, rtol, atol):
@@ -157,7 +88,7 @@ def moe_c3(hpc, dev, iters=10, parity_tokens=(4095,), cfg=None):
     byts = wbytes + T * H + T * H * 2
     out = {"workload": f"FusedMoE fp8 blockwise T={T} top{K} E={E} H={H} I={I} (BASELINE configs[2])",
            "ms": ms, "tok_per_s": T / ms * 1e3, "tflops": flops / ms / 1e9,
-           "frac_fp8_nominal_4500": flops / ms / 1e9 / FP8_NOMINAL_TFLOPS,
+           "frac_fp8_nominal_4500": flops / ms / 1e9 / FP8_TFLOPS,
            "frac_fp8_2x_measured_bf16": flops / ms / 1e9 / pk["fp8_tflops_2x_bf16"],
            "hbm_gbs": byts / ms / 1e6, "frac_hbm": byts / ms / 1e6 / pk["hbm_gbs"],
            "algorithmic_flops": flops, "algorithmic_bytes": byts, "launches_per_call": 5,
@@ -237,7 +168,7 @@ def prefill_c4(hpc, dev, kpt, iters=10, parity_items=None, cfg=None):
                        f"({'q,k per token/head, v per head' if kpt else 'q per token/head, kv per tensor'})"
                        " (BASELINE configs[3])",
            "ms": ms, "tok_per_s": S / ms * 1e3, "active_tiles": active, "tflops": flops / ms / 1e9,
-           "frac_fp8_nominal_4500": flops / ms / 1e9 / FP8_NOMINAL_TFLOPS,
+           "frac_fp8_nominal_4500": flops / ms / 1e9 / FP8_TFLOPS,
            "frac_fp8_2x_measured_bf16": flops / ms / 1e9 / pk["fp8_tflops_2x_bf16"],
            "algorithmic_flops": flops, "launches_per_call": 1,
            "timing": f"eager launches, {iters} calls, CUDA events"}

@@ -14,11 +14,10 @@ from pathlib import Path
 REPO = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(REPO))
 sys.path.insert(0, str(REPO / "hpc-ops_b200"))
-sys.path.insert(0, str(REPO / "tools"))
 import torch  # noqa: E402
 
 import hpc  # noqa: E402
-from bench_extras import peaks, time_eager  # noqa: E402
+from timing import card, peaks, time_eager  # noqa: E402
 
 
 def main():
@@ -32,7 +31,7 @@ def main():
     dev = "cuda"
     B, hq, hkv, D = a.batch, a.hq, a.hkv, 128
     pk = peaks()
-    out = {"batch": B, "ctx": a.ctx, "hq": hq, "hkv": hkv}
+    out = {"card": card(), "batch": B, "ctx": a.ctx, "hq": hq, "hkv": hkv}
     for bs in (64, 16):
         nb = (a.ctx + bs - 1) // bs
         g = torch.Generator(device=dev).manual_seed(0)

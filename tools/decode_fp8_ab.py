@@ -9,8 +9,10 @@ hpc/_C.so; everything that compares outputs runs there in a subprocess of its ow
     NHD and HND caches (NHD at rows <= 16 takes the rotated walk); np.array_equal
   * C2: `bench.py --no-extra` alternated between the builds `--reps` times each (step time, kernel
     time, tokens/s); the first run of each also dumps its output, compared bit for bit
-  * kernel time of hpc_attention_decode_fp8_partial_async at tools/decode_sweep.py's shapes, both
-    libraries loaded side by side in one process, alternated
+  * sweep: kernel time of hpc_attention_decode_fp8_partial_async at C2 (B 64, Hq 32, Hkv 8, 8192
+    tokens each) on NHD and HND caches, both libraries loaded side by side in one process,
+    alternated. With `--parts sweep --base hpc-ops_b200/hpc/_C.so` both arms are the current
+    build: its NHD and HND kernel times.
 One JSON document goes to stdout and to DIR/decode_fp8_ab_<parts>.json.
 """
 import argparse
@@ -22,6 +24,8 @@ import subprocess
 import sys
 import tempfile
 from pathlib import Path
+
+from timing import card, time_eager
 
 REPO = Path(__file__).resolve().parents[1]
 PKG = REPO / "hpc-ops_b200"
@@ -88,7 +92,7 @@ def compare_dirs(a: Path, b: Path):
 
 
 def sweep(base_so: Path, iters: int, reps: int):
-    """Kernel time at decode_sweep.py's shapes, both libraries in this process, alternated."""
+    """Kernel time at C2 on NHD and HND caches, both libraries in this process, alternated."""
     import ctypes
 
     sys.path.insert(0, str(REPO))
@@ -107,18 +111,6 @@ def sweep(base_so: Path, iters: int, reps: int):
     fns = {"base": fb, "new": _ffi.lib.hpc_attention_decode_fp8_partial_async}
     B, Sq, Hkv, Hq, S, MPL = 64, 1, 8, 32, 8192, 64
 
-    def timed(fn, args):
-        for _ in range(5):
-            _ffi.check(fn(*args))
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(iters):
-            fn(*args)
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / iters
-
     rows = []
     for layout in ("NHD", "HND"):
         d = sd.make_decode_fp8_inputs(B, Sq, [S] * B, Hkv, Hq, seed=41, layout=layout, device="cuda")
@@ -129,10 +121,12 @@ def sweep(base_so: Path, iters: int, reps: int):
         _, args, keep = hatt._decode_fp8_prepare(d["q"], kc, vc, d["block_ids"], d["kv_lens_total"],
                                                  d["q_scale"], d["k_scale"], d["v_scale"], Sq - 1,
                                                  True, 1, True, tm, None, out)
+        for fn in fns.values():
+            _ffi.check(fn(*args))
         t = {k: [] for k in fns}
         for _ in range(reps):
             for k, fn in fns.items():
-                t[k].append(timed(fn, args))
+                t[k].append(time_eager(lambda: fn(*args), iters, warm=5))
         r = {"layout": layout}
         for k, v in t.items():
             r[k + "_ms"] = statistics.median(v)
@@ -169,10 +163,7 @@ def main():
         worker(Path(a.worker))
         return
 
-    res = {}
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm",
-                        "--format=csv,noheader"], capture_output=True, text=True)
-    res["card"] = q.stdout.strip()
+    res = {"card": card()}
     with tempfile.TemporaryDirectory() as td:
         tmp = Path(td)
         arms = {"base": make_arm(tmp, "base", Path(a.base)), "new": make_arm(tmp, "new", Path(a.new))}

@@ -11,9 +11,10 @@ never sets it), each variant into its own shared library under build/probe/:
             the TMA stream alone takes, i.e. the ceiling of this access pattern on the card
   consumer  the producer signals each stage without loading it (the ring is zeroed once): the time
             the warpgroup's per-tile path alone takes
-Each is timed like tools/decode_sweep.py times hpc_attention_decode_fp8_partial_async (CUDA events
-over back-to-back launches), alternating with the normal kernel of hpc/_C.so; medians are printed
-as one JSON line. The kernel is HBM-bound when consumer < normal and normal is close to producer.
+Each is timed like `tools/decode_fp8_ab.py --parts sweep` times
+hpc_attention_decode_fp8_partial_async (CUDA events over back-to-back launches), alternating with
+the normal kernel of hpc/_C.so; medians are printed as one JSON line with the card they were
+measured on. The kernel is HBM-bound when consumer < normal and normal is close to producer.
 """
 import argparse
 import ctypes
@@ -81,6 +82,7 @@ def main():
     from hpc import _ffi
     from hpc import attention as hatt
     from synth.decode import make_decode_fp8_inputs
+    from timing import card, time_eager
 
     B, Sq, Hkv, Hq, S, MPL = 64, 1, 8, 32, 8192, 64  # C2
     d = make_decode_fp8_inputs(B, Sq, [S] * B, Hkv, Hq, seed=41, device="cuda")
@@ -100,25 +102,14 @@ def main():
         fn.restype = ctypes.c_int
         fn.argtypes = _ffi.lib.hpc_attention_decode_fp8_async.argtypes
         fns[name] = fn
-
-    def timed(fn):
-        for _ in range(10):
-            _ffi.check(fn(*args))
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(a.iters):
-            fn(*args)
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / a.iters
-
+    for fn in fns.values():
+        _ffi.check(fn(*args))
     runs = {k: [] for k in fns}
     for _ in range(a.reps):
         for k, fn in fns.items():
-            runs[k].append(timed(fn))
+            runs[k].append(time_eager(lambda: fn(*args), a.iters, warm=10))
     alg = B * Hkv * S * 2 * 128  # K and V bytes of the step
-    res = {"gpu": torch.cuda.get_device_name(0), "shape": "C2", "iters": a.iters}
+    res = {"card": card(), "shape": "C2", "iters": a.iters}
     for k, v in runs.items():
         med = statistics.median(v)
         res[k] = {"ms_median": med, "ms_min": min(v), "ms_max": max(v), "tb_s": alg / med / 1e9}

@@ -11,11 +11,10 @@ from pathlib import Path
 REPO = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(REPO))
 sys.path.insert(0, str(REPO / "hpc-ops_b200"))
-sys.path.insert(0, str(REPO / "tools"))
 import torch  # noqa: E402
 
 import hpc  # noqa: E402
-from bench_extras import peaks, time_eager  # noqa: E402
+from timing import card, peaks, time_eager  # noqa: E402
 
 
 def main():
@@ -23,7 +22,7 @@ def main():
     B, ctx, hq, hkv, D, bs = 64, 8192, 32, 8, 128, 64
     nb = ctx // bs
     pk = peaks()
-    out = {}
+    out = {"card": card()}
     g = torch.Generator(device=dev).manual_seed(0)
     ids = torch.randperm(B * nb, device=dev).to(torch.int32).view(B, nb)
     lens = torch.full((B,), ctx, dtype=torch.int32, device=dev)

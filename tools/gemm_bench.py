@@ -14,6 +14,7 @@ sys.path.insert(0, str(REPO / "hpc-ops_b200"))
 import torch  # noqa: E402
 
 import hpc  # noqa: E402
+from timing import card, time_graph  # noqa: E402
 
 
 def _time(fn, iters, flush):
@@ -32,38 +33,12 @@ def _time(fn, iters, flush):
     return tot / iters * 1e3  # us
 
 
-def _time_graph(fn, reps=20, iters=5):
-    """Kernel-side time per call: `reps` back-to-back calls captured in one CUDA graph (the
-    reference's benchmark harness times graphs as well), so host launch overhead is excluded."""
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            fn()
-    torch.cuda.current_stream().wait_stream(s)
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        for _ in range(reps):
-            fn()
-    g.replay()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        g.replay()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / (iters * reps) * 1e3
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--n", type=int, default=192)
     ap.add_argument("--k", type=int, default=4096)
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--out", default="")
-    ap.add_argument("--only-m", type=int, default=0, help="one M only, eager launches (for ncu)")
     a = ap.parse_args()
     torch.manual_seed(10086)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
@@ -73,12 +48,8 @@ def main():
     w_high = w.to(torch.bfloat16)
     w_low = ((w - w_high.float()) / scale).to(torch.bfloat16)
     rows = []
-    if a.only_m:
-        x = torch.randn(a.only_m, a.k, device="cuda", dtype=torch.float32).to(torch.bfloat16)
-        for _ in range(10):
-            hpc.gemm_bf16xfp32(x, w_high, w_low, scale, True, True, ws)
-        torch.cuda.synchronize()
-        return
+    gpu = card()
+    print(json.dumps({"card": gpu}))
     for m in [2, 4, 8, 16, 48, 96, 208, 512, 1024, 2048, 4096]:
         x = torch.randn(m, a.k, device="cuda", dtype=torch.float32).to(torch.bfloat16)
         xf = x.float()
@@ -91,7 +62,7 @@ def main():
         f_hpc = lambda: hpc.gemm_bf16xfp32(x, w_high, w_low, scale, True, True, ws)  # noqa: E731
         f_t = lambda: torch.matmul(xf, w.t())  # noqa: E731
         try:
-            gus, gus_t = _time_graph(f_hpc), _time_graph(f_t)
+            gus, gus_t = time_graph(f_hpc) * 1e3, time_graph(f_t) * 1e3
         except Exception as ex:  # noqa: BLE001
             print("graph timing failed:", ex)
             gus = gus_t = float("nan")
@@ -103,7 +74,7 @@ def main():
                      "gbps_graph": byts / gus / 1e3, "rel_err_vs_fp64": err})
         print(json.dumps(rows[-1]))
     if a.out:
-        Path(a.out).write_text(json.dumps({"n": a.n, "k": a.k, "rows": rows}, indent=1))
+        Path(a.out).write_text(json.dumps({"card": gpu, "n": a.n, "k": a.k, "rows": rows}, indent=1))
 
 
 if __name__ == "__main__":

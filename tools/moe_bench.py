@@ -1,4 +1,5 @@
-"""Time the FusedMoE blockwise pipeline at BASELINE config C3 (and its kernels). GPU box only.
+"""Time the FusedMoE blockwise pipeline at BASELINE config C3, or another shape, with the sampled
+oracle parity check of bench.py's `moe_c3` entry (tools/bench_extras.py). Needs a GPU.
 
     python tools/moe_bench.py [--tokens 4096] [--experts 128] [--topk 8] [--hidden 4096] [--inter 14336]
 """
@@ -12,7 +13,9 @@ sys.path.insert(0, str(REPO))
 sys.path.insert(0, str(REPO / "hpc-ops_b200"))
 import torch  # noqa: E402
 
+import bench_extras as bx  # noqa: E402
 import hpc  # noqa: E402
+from timing import card  # noqa: E402
 
 
 def main():
@@ -24,48 +27,9 @@ def main():
     ap.add_argument("--inter", type=int, default=14336)
     ap.add_argument("--iters", type=int, default=10)
     a = ap.parse_args()
-    dev = "cuda"
-    g = torch.Generator(device=dev).manual_seed(41)
-    T, E, K, H, I = a.tokens, a.experts, a.topk, a.hidden, a.inter
-    ids = torch.multinomial(torch.ones((T, E), device=dev), K, generator=g).to(torch.int32)
-    ids, _ = torch.sort(ids, dim=1)
-    ts = torch.rand((T, K), generator=g, device=dev)
-    ts = ts / ts.sum(1, keepdim=True)
-    x = (torch.randn((T, H), generator=g, device=dev) / 100).to(torch.float8_e4m3fn)
-    xs = torch.rand((T, H // 128), generator=g, device=dev) + 0.5
-
-    def w8(shape):
-        w = torch.empty(shape, dtype=torch.float8_e4m3fn, device=dev)
-        for e in range(shape[0]):
-            w[e] = torch.randn(shape[1:], generator=g, device=dev).to(torch.float8_e4m3fn)
-        return w
-
-    guw = w8((E, 2 * I, H))
-    dw = w8((E, H, I))
-    guws = torch.rand((E, 2 * I // 128, (H // 128 + 3) // 4 * 4), generator=g, device=dev) * 0.02
-    dws = torch.rand((E, H // 128, (I // 128 + 3) // 4 * 4), generator=g, device=dev) * 0.02
-
-    def run():
-        return hpc.fuse_moe_blockwise_fp8(x, xs, guw, guws, dw, dws, ids, ts, 0, E)
-
-    y = run()
-    torch.cuda.synchronize()
-    assert torch.isfinite(y.float()).all()
-    for _ in range(2):
-        run()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(a.iters):
-        run()
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / a.iters
-    flops = 2 * T * K * (2 * I * H + H * I)
-    wbytes = E * (2 * I * H + H * I)
-    out = {"ms": ms, "tok_per_s": T / ms * 1e3, "tflops": flops / ms / 1e9,
-           "frac_fp8_4500": flops / ms / 1e9 / 4500, "weight_gbs": wbytes / ms / 1e6, "cfg": vars(a)}
-    print(json.dumps(out))
+    cfg = dict(tokens=a.tokens, topk=a.topk, experts=a.experts, hidden=a.hidden, inter=a.inter)
+    res = bx.moe_c3(hpc, torch.device("cuda", 0), a.iters, parity_tokens=(a.tokens - 1,), cfg=cfg)
+    print(json.dumps({"card": card(), **res}))
 
 
 if __name__ == "__main__":

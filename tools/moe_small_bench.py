@@ -12,11 +12,10 @@ from pathlib import Path
 REPO = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(REPO))
 sys.path.insert(0, str(REPO / "hpc-ops_b200"))
-sys.path.insert(0, str(REPO / "tools"))
 import torch  # noqa: E402
 
 import hpc  # noqa: E402
-from bench_extras import peaks, time_graph  # noqa: E402
+from timing import card, peaks, time_graph  # noqa: E402
 
 
 def main():
@@ -50,8 +49,8 @@ def main():
     touched = int(torch.unique(ids).numel())
     wbytes = touched * 3 * I * H
     pk = peaks()
-    print(json.dumps({"us": ms * 1e3, "experts_touched": touched, "rows_per_expert_avg": T * K / E,
-                      "weight_bytes": wbytes, "hbm_floor_us": wbytes / pk["hbm_gbs"] / 1e3,
+    print(json.dumps({"card": card(), "us": ms * 1e3, "experts_touched": touched,
+                      "rows_per_expert_avg": T * K / E, "weight_bytes": wbytes, "hbm_floor_us": wbytes / pk["hbm_gbs"] / 1e3,
                       "frac_of_hbm_floor": (wbytes / pk["hbm_gbs"] / 1e3) / (ms * 1e3),
                       "tok_per_s": T / ms * 1e3, "cfg": vars(a),
                       "timing": "CUDA-graph replay, 10 calls per graph x 5 replays"}))

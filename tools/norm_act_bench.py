@@ -14,7 +14,6 @@ H = 1024 (one warp per row; 4096 takes four and 5120 / 7168 eight); masked ops a
 C 2048 with 100 %, 50 % and 10 % of the rows valid, per-tensor and blockwise."""
 import argparse
 import json
-import subprocess
 import sys
 from pathlib import Path
 
@@ -24,39 +23,14 @@ sys.path.insert(0, str(REPO / "hpc-ops_b200"))
 import torch  # noqa: E402
 
 import hpc  # noqa: E402
+from timing import HBM_GBS, card, spread, time_graph  # noqa: E402
 
-HBM = 3.35e12
-
-
-def graphed(fn):
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(3):
-            fn()
-    torch.cuda.current_stream().wait_stream(s)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        fn()
-    return g.replay
+HBM = HBM_GBS * 1e9
 
 
-def timed(fn, iters):
-    for _ in range(5):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / iters * 1e3  # us
-
-
-def spread(fn, iters, reps):
-    t = sorted(timed(fn, iters) for _ in range(reps))
-    return t[len(t) // 2], t[0], t[-1]
+def graphed_us(fn, a):
+    """Median, min and max in µs of `a.reps` windows of `a.iters` replays of a graph of one call."""
+    return [t * 1e3 for t in spread(lambda: time_graph(fn, 1, a.iters), a.reps)]
 
 
 def torch_rmsnorm(x, w, sc, eps, is_moe):
@@ -96,10 +70,8 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--json", default=None)
     a = ap.parse_args()
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm",
-                           "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    print("card:", card, flush=True)
-    res = {"card": card, "rows": []}
+    res = {"card": card(), "rows": []}
+    print(json.dumps({"card": res["card"]}), flush=True)
     eps = 1e-6
     sc = torch.tensor([0.05, 0.5], device="cuda")
     shapes = [(T, H) for H in (4096, 5120, 7168) for T in (1, 16, 128, 1024, 8192, 32768)]
@@ -108,11 +80,11 @@ def main():
         x = torch.randn(T, H, device="cuda").to(torch.bfloat16)
         w = torch.rand(H, device="cuda").to(torch.bfloat16)
         for moe in (False, True):
-            ours = graphed(lambda: hpc.fused_rmsnorm_with_scale(x, w, eps, sc, moe))
-            ref = graphed(lambda: torch_rmsnorm(x, w, sc, eps, moe))
+            ours = lambda: hpc.fused_rmsnorm_with_scale(x, w, eps, sc, moe)  # noqa: E731
+            ref = lambda: torch_rmsnorm(x, w, sc, eps, moe)  # noqa: E731
             by = T * H * 2 + H * 2 + T * H * (6 if moe else 1)
-            res["rows"].append(row("rmsnorm", by, spread(ours, a.iters, a.reps),
-                                   spread(ref, a.iters, a.reps), T=T, H=H, is_moe=moe))
+            res["rows"].append(row("rmsnorm", by, graphed_us(ours, a), graphed_us(ref, a),
+                                   T=T, H=H, is_moe=moe))
         del x
     E, T, C = 32, 1024, 2048
     gu = torch.randn(E * T, 2 * C, device="cuda").to(torch.bfloat16)
@@ -123,13 +95,13 @@ def main():
         valid = E * int(T * fill)
         for blockwise in (False, True):
             if blockwise:
-                ours = graphed(lambda: hpc.masked_act_mul_and_blockwise_quant(gu, cnt, out, osc))
+                ours = lambda: hpc.masked_act_mul_and_blockwise_quant(gu, cnt, out, osc)  # noqa: E731
             else:
-                ours = graphed(lambda: hpc.masked_act_mul_and_quant(gu, sc[:1], cnt, out))
-            ref = graphed(lambda: torch_masked(gu, cnt, T, sc, blockwise))
+                ours = lambda: hpc.masked_act_mul_and_quant(gu, sc[:1], cnt, out)  # noqa: E731
+            ref = lambda: torch_masked(gu, cnt, T, sc, blockwise)  # noqa: E731
             by = valid * (4 * C + C + (4 * C // 128 if blockwise else 0))
             res["rows"].append(row("masked_blockwise" if blockwise else "masked_pertensor", by,
-                                   spread(ours, a.iters, a.reps), spread(ref, a.iters, a.reps),
+                                   graphed_us(ours, a), graphed_us(ref, a),
                                    E=E, T_max=T, C=C, fill=fill))
     if a.json:
         Path(a.json).parent.mkdir(parents=True, exist_ok=True)

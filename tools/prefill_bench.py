@@ -1,5 +1,6 @@
 """Time the FP8 block-sparse prefill at BASELINE config C4 (B=1, seq=32768, GQA 32/8, d=128,
-25 % of causal 128x128 tiles + diagonal). GPU box only.
+25 % of causal 128x128 tiles + diagonal), or another shape, with the sampled oracle parity check of
+bench.py's `prefill_c4_*` entries (tools/bench_extras.py). Needs a GPU.
 
     python tools/prefill_bench.py [--seq 32768] [--skip 0.75] [--kpt 1]
 """
@@ -13,8 +14,9 @@ sys.path.insert(0, str(REPO))
 sys.path.insert(0, str(REPO / "hpc-ops_b200"))
 import torch  # noqa: E402
 
+import bench_extras as bx  # noqa: E402
 import hpc  # noqa: E402
-from synth import prefill as op  # noqa: E402
+from timing import card  # noqa: E402
 
 
 def main():
@@ -26,35 +28,9 @@ def main():
     ap.add_argument("--kpt", type=int, default=1)
     ap.add_argument("--iters", type=int, default=10)
     a = ap.parse_args()
-    d = op.make_inputs([a.seq], [a.seq], a.hq, a.hkv, a.skip, bool(a.kpt), device="cuda")
-    mask = d["block_mask"].to(torch.uint8).contiguous()
-    qt = (hpc.QuantType.QPERTOKEN_PERHEAD_KPERTOKEN_PERHEAD_VPERHEAD if a.kpt
-          else hpc.QuantType.QPERTOKEN_PERHEAD_KPERTENSOR_VPERTENSOR)
-
-    def run():
-        return hpc.attention_with_kvcache_blocksparse_prefill_fp8(
-            d["q"], d["kcache"], d["vcache"], d["qscale"], d["kscale"], d["vscale"],
-            d["cu_seqlens_q"], d["block_ids"], d["seqlens_kv"], d["max_q"], quant_type=qt,
-            block_mask=mask)
-
-    y = run()
-    torch.cuda.synchronize()
-    assert torch.isfinite(y.float()).all()
-    for _ in range(2):
-        run()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(a.iters):
-        run()
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / a.iters
-    active = int(mask.sum().item())
-    flops = active * 4 * 128 ** 3
-    print(json.dumps({"ms": ms, "active_tiles": active, "tflops": flops / ms / 1e9,
-                      "frac_fp8_4500": flops / ms / 1e9 / 4500, "tok_per_s": a.seq / ms * 1e3,
-                      "cfg": vars(a)}))
+    cfg = dict(seq=a.seq, hq=a.hq, hkv=a.hkv, skip=a.skip)
+    res = bx.prefill_c4(hpc, torch.device("cuda", 0), bool(a.kpt), a.iters, cfg=cfg)
+    print(json.dumps({"card": card(), **res}))
 
 
 if __name__ == "__main__":

@@ -12,7 +12,6 @@ power limit and max SM clock first.
 import argparse
 import json
 import math
-import subprocess
 import sys
 from pathlib import Path
 
@@ -24,25 +23,7 @@ from torch.nn.attention import SDPBackend, sdpa_kernel  # noqa: E402
 
 import hpc  # noqa: E402
 from synth import prefill_bf16 as sb  # noqa: E402
-
-PEAK = 989e12
-
-
-def card():
-    out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm",
-                          "--format=csv,noheader"], capture_output=True, text=True).stdout
-    name, power, clock = [s.strip() for s in out.splitlines()[0].split(",")]
-    return dict(card=name, power_limit=power, max_sm_clock=clock)
-
-
-def timed(fn, iters):
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b) / iters
+from timing import BF16_TFLOPS, card, time_eager  # noqa: E402
 
 
 def pairs(q_lens, kv_lens):
@@ -64,15 +45,14 @@ def run_shape(name, d, q_lens, kv_lens, args, sdpa=None):
     for f in fns:
         for _ in range(args.warmup):
             f()
-    torch.cuda.synchronize()
     times = [[] for _ in fns]
     for _ in range(args.rounds):
         for i, f in enumerate(fns):
-            times[i].append(timed(f, args.iters))
+            times[i].append(time_eager(f, args.iters, warm=0))
     med = [sorted(t)[len(t) // 2] for t in times]
     flop = 4 * 128 * hq * pairs(q_lens, kv_lens)
     res = dict(shape=name, ms=round(med[0], 4), tflops=round(flop / med[0] / 1e9, 1),
-               share_of_989=round(flop / med[0] / 1e-3 / PEAK, 3))
+               share_of_989=round(flop / med[0] / 1e9 / BF16_TFLOPS, 3))
     if sdpa:
         y, ys = ours(), sdpa()
         diff = (y.float() - ys.transpose(0, 1).float()).abs().max()
@@ -88,7 +68,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a GPU"
-    print(json.dumps(card()), flush=True)
+    print(json.dumps({"card": card()}), flush=True)
     hq, hkv = 32, 8
     for seq in (8192, 16384, 32768):
         d = sb.make_reference_case("dense", [seq], hq=hq, hkv=hkv, seed=seq, device="cuda")

@@ -11,11 +11,10 @@ from pathlib import Path
 REPO = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(REPO))
 sys.path.insert(0, str(REPO / "hpc-ops_b200"))
-sys.path.insert(0, str(REPO / "tools"))
 import torch  # noqa: E402
 
 import hpc  # noqa: E402
-from bench_extras import peaks, time_eager  # noqa: E402
+from timing import card, peaks, time_eager  # noqa: E402
 
 
 def main():
@@ -54,7 +53,7 @@ def main():
         byts = T * (hq + 2 * hkv) * D * 2 + T * (hq + 2 * hkv) * D * ob + T * D * 4 + (T * hq * 4 if fp8 else 0)
         res[name] = {"ms": ms, "gbs": byts / ms / 1e6, "frac_hbm": byts / ms / 1e6 / pk["hbm_gbs"],
                      "algorithmic_bytes": byts, "tok_per_s": T / ms * 1e3}
-    print(json.dumps({"rows": T, "hq": hq, "hkv": hkv, **res}))
+    print(json.dumps({"card": card(), "rows": T, "hq": hq, "hkv": hkv, **res}))
 
 
 if __name__ == "__main__":

@@ -12,19 +12,17 @@ GPU only.
 """
 import argparse
 import json
-import subprocess
 import sys
 from pathlib import Path
 
 REPO = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(REPO))
 sys.path.insert(0, str(REPO / "hpc-ops_b200"))
-sys.path.insert(0, str(REPO / "tools"))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 import hpc  # noqa: E402
-from bench_extras import peaks, time_graph  # noqa: E402
+from timing import card, peaks, time_graph  # noqa: E402
 
 V = 120832
 T, RP, TOPK, TOPP = 0.7, 1.05, 20, 0.9
@@ -61,8 +59,7 @@ def main():
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     assert torch.cuda.is_available(), "sampler_bench needs a GPU"
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                          capture_output=True, text=True).stdout.strip().splitlines()[0]
+    gpu = card()
     hbm = peaks()["hbm_gbs"]
     rows = []
     for B in [int(b) for b in a.batches.split(",")]:
@@ -90,11 +87,11 @@ def main():
                              hbm_share=round(nbytes / (ms * 1e-3) / (hbm * 1e9), 3),
                              torch_us=round(ms_torch * 1e3, 2), speedup=round(ms_torch / ms, 2)))
             print(json.dumps(rows[-1]), flush=True)
-    res = dict(card=card, vocab=V, hbm_gbs=hbm, rows=rows)
+    res = dict(card=gpu, vocab=V, hbm_gbs=hbm, rows=rows)
     if a.out:
         Path(a.out).parent.mkdir(parents=True, exist_ok=True)
         Path(a.out).write_text(json.dumps(res, indent=1))
-    print(json.dumps(dict(card=card)))
+    print(json.dumps(dict(card=gpu)))
 
 
 if __name__ == "__main__":

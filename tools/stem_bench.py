@@ -11,7 +11,6 @@ torch ops (the two prep stages, and GEMM + TPD, each timed under CUDA-graph repl
 card name and power limit are read in the same run."""
 import argparse
 import json
-import subprocess
 import sys
 from pathlib import Path
 
@@ -21,22 +20,10 @@ sys.path.insert(0, str(REPO / "hpc-ops_b200"))
 import torch  # noqa: E402
 
 import hpc  # noqa: E402
+from timing import BF16_TFLOPS, HBM_GBS, card, spread, time_eager, time_graph  # noqa: E402
 
-HBM = 3.35e12
-BF16 = 989e12
-
-
-def timed(fn, iters, warm=5):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / iters * 1e3  # us
+HBM = HBM_GBS * 1e9
+BF16 = BF16_TFLOPS * 1e12
 
 
 def inputs(q_len, kv_len, hq, hkv, quant, seed=0):
@@ -83,24 +70,6 @@ def torch_prep(d, kv_len, q_len):
     return kflat.bfloat16(), vbias, qflat.bfloat16()
 
 
-def graphed(fn):
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        fn()
-    torch.cuda.current_stream().wait_stream(s)
-    gr = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(gr):
-        fn()
-    return gr.replay
-
-
-def spread(fn, iters, reps):
-    """Median, min and max over `reps` timings of `iters` launches each."""
-    t = sorted(timed(fn, iters) for _ in range(reps))
-    return t[len(t) // 2], t[0], t[-1]
-
-
 def torch_stages(off, kflat, vbias, qflat):
     """The GEMM + TPD stages as torch ops (topk by value instead of the exact threshold)."""
     hq, hkv = qflat.shape[1], kflat.shape[1]
@@ -120,10 +89,12 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--json", default=None)
     a = ap.parse_args()
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm",
-                           "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    print("card:", card)
-    res = {"card": card, "rows": []}
+    res = {"card": card(), "rows": []}
+    print(json.dumps({"card": res["card"]}))
+
+    def us(timer):  # median, min, max in µs of a.reps windows
+        return [t * 1e3 for t in spread(timer, a.reps)]
+
     for name, q_len, kv_len in (("C4", 32768, 32768), ("chunked", 8192, 24576)):
         for quant in (1, 0):
             d = inputs(q_len, kv_len, 32, 8, quant)
@@ -156,15 +127,15 @@ def main():
             }
             # the same stages as torch ops, replayed from CUDA graphs
             off = (kv_len - q_len + 127) // 128
-            t_torch = spread(graphed(lambda: torch_stages(off, kflat, vbias, qflat)), a.iters, a.reps)
-            t_torch_prep = spread(graphed(lambda: torch_prep(d, kv_len, q_len)), a.iters, a.reps)
+            t_torch = us(lambda: time_graph(lambda: torch_stages(off, kflat, vbias, qflat), 1, a.iters))
+            t_torch_prep = us(lambda: time_graph(lambda: torch_prep(d, kv_len, q_len), 1, a.iters))
             prefill = lambda: hpc.attention_with_kvcache_blocksparse_prefill_fp8(
                 d["q"], d["kc"], d["vc"], d["qscale"], d["ks"], d["vs"], d["cu"], d["ids"], d["kvl"],
                 q_len, qt, block_mask=mask)
-            t_prefill = timed(prefill, max(5, a.iters // 5))
+            t_prefill = time_eager(prefill, max(5, a.iters // 5)) * 1e3
             for stage, fn in (("prep_kv", prep_kv), ("prep_q", prep_q), ("gemm", gemm), ("tpd", tpd),
                               ("stem_paged_kv", full)):
-                t, lo, hi = spread(fn, a.iters, a.reps)
+                t, lo, hi = us(lambda: time_eager(fn, a.iters))
                 by, fl = model[stage]
                 floor = max(by / HBM, fl / BF16) * 1e6
                 row = dict(shape=name, quant=quant, stage=stage, us=round(t, 2), us_min=round(lo, 2),
