@@ -151,6 +151,10 @@ if hasattr(lib, "hpc_fused_rmsnorm_with_scale_async"):
     lib.hpc_masked_act_mul_and_blockwise_quant_async.restype = c_int
     lib.hpc_masked_act_mul_and_blockwise_quant_async.argtypes = [c_ptr] * 4 + [c_int] * 3 + [c_ptr]
 
+if hasattr(lib, "hpc_moe_topk_gating_async"):
+    lib.hpc_moe_topk_gating_async.restype = c_int
+    lib.hpc_moe_topk_gating_async.argtypes = [c_ptr] * 4 + [c_int] * 8 + [c_i64, c_f32, c_ptr]
+
 def check(rc: int, what: str = ""):
     """Turn a launcher status into the RuntimeError the reference raises via TORCH_CHECK."""
     if rc != 0:

@@ -3,7 +3,13 @@
 Host prep mirrors the reference entries (src/fuse_moe/entry.cc:269-639): validation, tile table,
 scratch allocation — except that the bf16 Gate-Up scratch is not allocated: this build fuses
 SiLU*mul + FP8 re-quant into the Gate-Up GEMM epilogue.
+
+`moe_topk_gating` (no reference counterpart) turns the route GEMM's logits into the topk_ids /
+topk_scale these operators consume.
 """
+from enum import IntEnum
+from typing import Optional
+
 import torch
 from torch import Tensor
 
@@ -323,3 +329,138 @@ def _fuse_moe_blockwise_fp8_fake(x, x_scale, gate_up_weight, gate_up_weight_scal
 @torch.library.register_fake("hpc::reduce")
 def _reduce_fake(x, topk_pos, topk_scale, shared_output):
     return torch.empty((topk_pos.shape[0], x.shape[1]), dtype=torch.bfloat16, device=x.device)
+
+
+class GatingScore(IntEnum):
+    """How moe_topk_gating turns a router logit into an expert score."""
+    SOFTMAX = 0
+    SIGMOID = 1
+
+
+MAX_GATING_EXPERTS = 512
+MAX_GATING_TOPK = 16
+
+
+def _check_gating(router_logits, topk, scoring, correction_bias, num_expert_group, topk_group,
+                  topk_ids, topk_weights):
+    """The launcher's limits, checked before any device work; returns (num_tokens, num_experts)."""
+    x = router_logits
+    _require(x.dim() == 2, f"moe_topk_gating: router_logits must be 2-D [T, E], got {tuple(x.shape)}")
+    _require(x.dtype in (torch.float32, torch.bfloat16),
+             f"moe_topk_gating: router_logits must be float32 or bfloat16, got {x.dtype}")
+    T, E = x.shape
+    _require(x.stride(1) == 1 or E == 1, "moe_topk_gating: router_logits rows must be contiguous")
+    _require(1 <= E <= MAX_GATING_EXPERTS,
+             f"moe_topk_gating: number of experts {E} outside [1, {MAX_GATING_EXPERTS}]")
+    _require(1 <= topk <= min(MAX_GATING_TOPK, E),
+             f"moe_topk_gating: topk {topk} outside [1, min({MAX_GATING_TOPK}, {E})]")
+    _require(int(scoring) in (0, 1), f"moe_topk_gating: unknown scoring {scoring}")
+    G = num_expert_group
+    _require(G >= 1 and E % G == 0,
+             f"moe_topk_gating: num_expert_group {G} must be positive and divide the {E} experts")
+    _require(1 <= topk_group <= G,
+             f"moe_topk_gating: topk_group {topk_group} outside [1, num_expert_group {G}]")
+    _require(topk <= topk_group * (E // G),
+             f"moe_topk_gating: topk {topk} exceeds the {topk_group * (E // G)} experts of "
+             f"topk_group {topk_group} groups")
+    esize = x.element_size()
+    if T > 1:
+        _require(x.stride(0) >= E and x.stride(0) * esize % 16 == 0,
+                 f"moe_topk_gating: row stride {x.stride(0)} elements must be at least the {E} "
+                 "experts and a multiple of 16 bytes")
+    if correction_bias is not None:
+        _require(correction_bias.dtype == torch.float32 and correction_bias.dim() == 1
+                 and correction_bias.numel() == E and correction_bias.is_contiguous(),
+                 f"moe_topk_gating: correction_bias must be a contiguous float32 tensor of {E} "
+                 "values")
+        _require(G == 1 or E // G >= 2,
+                 "moe_topk_gating: a correction bias with groups needs at least 2 experts per "
+                 "group (the group score is the sum of its top-2 keys)")
+    for t, name, dt in ((topk_ids, "topk_ids", torch.int32), (topk_weights, "topk_weights", torch.float32)):
+        if t is not None:
+            _require(t.dtype == dt and tuple(t.shape) == (T, topk) and t.is_contiguous(),
+                     f"moe_topk_gating: {name} must be a contiguous {dt} tensor of shape "
+                     f"[{T}, {topk}]")
+    _require(x.is_cuda, "moe_topk_gating: router_logits must be a CUDA tensor")
+    for t, name in ((correction_bias, "correction_bias"), (topk_ids, "topk_ids"),
+                    (topk_weights, "topk_weights")):
+        _require(t is None or t.device == x.device,
+                 f"moe_topk_gating: {name} must be on the device of router_logits")
+    _require(x.data_ptr() % 16 == 0, "moe_topk_gating: router_logits must be 16-byte aligned")
+    return T, E
+
+
+def _moe_topk_gating_impl(router_logits, topk, scoring, renormalize, correction_bias,
+                          num_expert_group, topk_group, routed_scaling_factor, topk_ids,
+                          topk_weights):
+    T, E = _check_gating(router_logits, topk, scoring, correction_bias, num_expert_group,
+                         topk_group, topk_ids, topk_weights)
+    dev = router_logits.device
+    if topk_ids is None:
+        topk_ids = torch.empty((T, topk), dtype=torch.int32, device=dev)
+    if topk_weights is None:
+        topk_weights = torch.empty((T, topk), dtype=torch.float32, device=dev)
+    if T == 0:
+        return topk_ids, topk_weights
+    _check_rc(_lib.hpc_moe_topk_gating_async(
+        _ptr(router_logits), _ptr(correction_bias), _ptr(topk_ids), _ptr(topk_weights), T, E,
+        0 if router_logits.dtype == torch.float32 else 1, int(topk), int(scoring),
+        int(bool(renormalize)), int(num_expert_group), int(topk_group), router_logits.stride(0),
+        float(routed_scaling_factor), _stream_of(router_logits)), "moe_topk_gating")
+    return topk_ids, topk_weights
+
+
+_ops.define(
+    "moe_topk_gating(Tensor router_logits, int topk, int scoring, bool renormalize, Tensor? "
+    "correction_bias, int num_expert_group, int topk_group, float routed_scaling_factor, Tensor? "
+    "topk_ids, Tensor? topk_weights) -> (Tensor, Tensor)")
+_ops.impl("moe_topk_gating", _moe_topk_gating_impl, "CUDA")
+
+
+def moe_topk_gating(router_logits: Tensor, topk: int, scoring: GatingScore = GatingScore.SOFTMAX,
+                    renormalize: bool = True, correction_bias: Optional[Tensor] = None,
+                    num_expert_group: int = 1, topk_group: int = 1,
+                    routed_scaling_factor: float = 1.0, topk_ids: Optional[Tensor] = None,
+                    topk_weights: Optional[Tensor] = None) -> tuple:
+    """Router logits -> (topk_ids int32 [T, topk], topk_weights float32 [T, topk]), the
+    topk_ids / topk_scale of fuse_moe*, in one sm_90a kernel.
+
+    router_logits [T, E] float32 or bfloat16 with contiguous rows and any 16-byte row stride, so
+    a column slice `logits[:, :E]` of a wider (padded) route-GEMM output is read in place.
+    Per token row, in fp32 (x_e = float(logits[t, e])):
+
+    1. Score s_e: SOFTMAX exp(x_e - max x) / sum_j exp(x_j - max x) over all E; SIGMOID
+       1 / (1 + exp(-x_e)).
+    2. Selection key c_e: x_e for SOFTMAX without a bias (the order of s_e, exactly: logits that
+       round to one fp32 score do not tie); otherwise s_e + correction_bias[e].
+    3. num_expert_group G > 1 (E % G == 0): group g is experts [g E/G, (g+1) E/G). Its score is
+       the sum of its top-2 keys with a bias, its max key without (vLLM's grouped_topk rule); the
+       topk_group best groups, by (score desc, group id asc), stay eligible.
+    4. The topk eligible experts in the order (key desc, id asc), NaN below -inf: every row's ids
+       are distinct and in [0, E) for any input (its weights are unspecified when it holds NaN),
+       and a -inf key is never chosen while a finite one is available.
+    5. Weights w_i = s_{id_i} (the unbiased score); with renormalize, w_i /= sum_i w_i summed in
+       rank order; then w_i *= routed_scaling_factor.
+    6. Outputs in rank order. Caller-given topk_ids / topk_weights (contiguous, [T, topk]) are
+       written in place and returned.
+
+    Limits: 1 <= E <= 512, 1 <= topk <= min(16, E), topk_group <= G, topk <= topk_group E / G,
+    groups of at least 2 experts with a bias, 16-byte aligned logits. T = 0 returns empty tensors
+    without a launch. No allocation beyond the outputs and no host synchronisation: the call can
+    be captured in a CUDA graph, and it chains to the following fuse_moe* launch by programmatic
+    dependent launch."""
+    return torch.ops.hpc.moe_topk_gating(router_logits, int(topk), int(scoring), bool(renormalize),
+                                         correction_bias, int(num_expert_group), int(topk_group),
+                                         float(routed_scaling_factor), topk_ids, topk_weights)
+
+
+@torch.library.register_fake("hpc::moe_topk_gating")
+def _moe_topk_gating_fake(router_logits, topk, scoring, renormalize, correction_bias,
+                          num_expert_group, topk_group, routed_scaling_factor, topk_ids,
+                          topk_weights):
+    T = router_logits.shape[0]
+    dev = router_logits.device
+    ids = topk_ids if topk_ids is not None else torch.empty((T, topk), dtype=torch.int32, device=dev)
+    w = (topk_weights if topk_weights is not None
+         else torch.empty((T, topk), dtype=torch.float32, device=dev))
+    return ids, w

@@ -200,6 +200,25 @@ int hpc_fused_rmsnorm_with_scale_async(const void* input_ptr, const void* weight
                                        float eps, int batch_size, int hidden_state, int is_moe,
                                        cudaStream_t stream);
 
+/* ---- MoE top-k gating -----------------------------------------------------------------------------
+ * No reference counterpart: turns router logits into the topk_ids / topk_scale that FusedMoE
+ * consumes. router_logits [num_tokens, num_experts] float32 (logits_dtype 0) or bfloat16 (1),
+ * elements of a row contiguous, row_stride elements between rows (>= num_experts, a multiple of
+ * 16 bytes; unused for a single row), 16-byte aligned base. scoring 0 = softmax over all experts,
+ * 1 = sigmoid. correction_bias f32 [num_experts] or NULL. Per row, in fp32: key = logit (softmax
+ * without bias) or score + bias; with num_expert_group G > 1 only the topk_group best groups
+ * (max key, or sum of the top-2 keys with a bias) are eligible; the topk largest keys, ties to the
+ * lower id, NaN below -inf, give topk_ids int32 [num_tokens, topk]; topk_weights f32
+ * [num_tokens, topk] = the unbiased scores, divided by their sum (rank order) when renormalize,
+ * then times routed_scaling_factor. 1 <= num_experts <= 512, 1 <= topk <= min(16, num_experts),
+ * num_experts % G == 0, topk_group <= G, topk <= topk_group * num_experts / G, groups of at least
+ * 2 experts with a bias. No allocation or host synchronisation: capturable. */
+int hpc_moe_topk_gating_async(const void* router_logits_ptr, const float* correction_bias_ptr,
+                              int* topk_ids_ptr, float* topk_weights_ptr, int num_tokens,
+                              int num_experts, int logits_dtype, int topk, int scoring,
+                              int renormalize, int num_expert_group, int topk_group,
+                              int64_t row_stride, float routed_scaling_factor, cudaStream_t stream);
+
 /* ---- FusedMoE -----------------------------------------------------------------------------------
  * replace reference src/fuse_moe/fuse_moe.h:15-62, argument for argument (bool -> int).
  * `intermediate_size` is gate_up_weight.size(1) (= 2*I) as in the reference entries.
