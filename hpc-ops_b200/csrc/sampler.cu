@@ -15,8 +15,7 @@
 
 #include <climits>
 
-#include "common.cuh"
-#include "host_utils.h"
+#include "sampler_common.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -25,7 +24,6 @@ namespace {
 
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
-constexpr int kMaxSlices = 8;
 constexpr unsigned kFull = 0xffffffffu;
 
 struct SamplerParams {
@@ -54,63 +52,11 @@ struct SamplerParams {
   int chunks_per_slice;  // 8-token chunks
 };
 
-// ---- Philox4x32-10 (Salmon et al., SC'11) --------------------------------------------------------
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
-#pragma unroll
-  for (int r = 0; r < 10; r++) {
-    const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
-    const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
-    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
-    k.x += 0x9E3779B9u;
-    k.y += 0xBB67AE85u;
-  }
-  return c;
-}
-
-// 23 random bits -> u in [2^-24, 1 - 2^-24], every value exact in fp32; g = -log(-log u) is finite.
-__device__ __forceinline__ float gumbel_of(uint32_t x) {
-  const float u = __fmaf_rn(static_cast<float>(x >> 9), 1.1920928955078125e-7f, 5.9604644775390625e-8f);
-  return -logf(-logf(u));
-}
-
-// Gumbel noise of tokens 4q .. 4q+3 of `row`
-__device__ __forceinline__ float4 philox_gumbel4(const SamplerParams& p, uint32_t q, int row,
-                                                 uint64_t offset) {
-  const uint4 r = philox4x32_10(
-      make_uint4(q, static_cast<uint32_t>(row), static_cast<uint32_t>(offset),
-                 static_cast<uint32_t>(offset >> 32)),
-      make_uint2(static_cast<uint32_t>(p.seed), static_cast<uint32_t>(p.seed >> 32)));
-  return make_float4(gumbel_of(r.x), gumbel_of(r.y), gumbel_of(r.z), gumbel_of(r.w));
-}
-
 __device__ __forceinline__ float noise_at(const SamplerParams& p, int row, int tok, uint64_t offset) {
   if (p.noise != nullptr) return p.noise[static_cast<int64_t>(row) * p.vocab + tok];
-  const float4 g = philox_gumbel4(p, static_cast<uint32_t>(tok) >> 2, row, offset);
+  const float4 g = philox_gumbel4(p.seed, static_cast<uint32_t>(tok) >> 2, row, offset);
   const int j = tok & 3;
   return j == 0 ? g.x : j == 1 ? g.y : j == 2 ? g.z : g.w;
-}
-
-// (value descending, token id ascending); NaN is never better
-__device__ __forceinline__ bool better(float a, int ia, float b, int ib) {
-  return a > b || (a == b && ia < ib);
-}
-
-template <typename T>
-__device__ __forceinline__ void load8(const T* row, int c, float (&x)[8]);
-template <>
-__device__ __forceinline__ void load8<float>(const float* row, int c, float (&x)[8]) {
-  const float4 a = ld_nc_f4(row + 8 * c), b = ld_nc_f4(row + 8 * c + 4);
-  x[0] = a.x, x[1] = a.y, x[2] = a.z, x[3] = a.w, x[4] = b.x, x[5] = b.y, x[6] = b.z, x[7] = b.w;
-}
-template <>
-__device__ __forceinline__ void load8<__nv_bfloat16>(const __nv_bfloat16* row, int c, float (&x)[8]) {
-  const uint4 v = ld_nc_v4(row + 8 * c);
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-  for (int i = 0; i < 4; i++) {
-    x[2 * i] = __uint_as_float(w[i] << 16);
-    x[2 * i + 1] = __uint_as_float(w[i] & 0xffff0000u);
-  }
 }
 
 struct RowScalars {
@@ -141,25 +87,6 @@ __device__ __forceinline__ void penalise_and_temper(const RowScalars& s, int c, 
   }
 }
 
-// The last CTA of the launch to get here advances the launch counter: every CTA has read the
-// offset before it arrives.
-__device__ __forceinline__ void advance_rng(const SamplerParams& p) {
-  if (p.rng_word == nullptr || threadIdx.x != 0) return;
-  __threadfence();
-  unsigned int* done = reinterpret_cast<unsigned int*>(p.rng_word + 1);
-  const unsigned int total = gridDim.x * gridDim.y;
-  if (atomicAdd(done, 1u) == total - 1) {
-    p.rng_word[0] += 1;
-    *done = 0;
-    __threadfence();
-  }
-}
-
-__device__ __forceinline__ uint64_t launch_offset(const SamplerParams& p) {
-  return p.rng_word != nullptr ? p.rng_base + *reinterpret_cast<volatile unsigned long long*>(p.rng_word)
-                               : 0;
-}
-
 // ================================ temperature-only fast path ======================================
 __device__ __forceinline__ void argmax_step(float s, int id, float& best, int& best_id) {
   if (better(s, id, best, best_id)) best = s, best_id = id;
@@ -173,7 +100,7 @@ __global__ void __launch_bounds__(kThreads) sampler_temperature_kernel(const Sam
   const int b = blockIdx.y;
   const int slice = static_cast<int>(cluster.block_rank());
   pdl_wait();
-  const uint64_t offset = launch_offset(p);
+  const uint64_t offset = launch_offset(p.rng_word, p.rng_base);
   const T* row = static_cast<const T*>(p.logits) + b * p.row_stride;
   const float temp = p.temp != nullptr ? p.temp[b] : p.temp_val;
   const bool sample = temp > 0.f;  // false for t <= 0 and NaN: plain argmax
@@ -195,7 +122,7 @@ __global__ void __launch_bounds__(kThreads) sampler_temperature_kernel(const Sam
         const float4 a = ld_nc_f4(noise_row + 8 * c), e = ld_nc_f4(noise_row + 8 * c + 4);
         g[0] = a.x, g[1] = a.y, g[2] = a.z, g[3] = a.w, g[4] = e.x, g[5] = e.y, g[6] = e.z, g[7] = e.w;
       } else {
-        const float4 a = philox_gumbel4(p, 2 * c, b, offset), e = philox_gumbel4(p, 2 * c + 1, b, offset);
+        const float4 a = philox_gumbel4(p.seed, 2 * c, b, offset), e = philox_gumbel4(p.seed, 2 * c + 1, b, offset);
         g[0] = a.x, g[1] = a.y, g[2] = a.z, g[3] = a.w, g[4] = e.x, g[5] = e.y, g[6] = e.z, g[7] = e.w;
       }
 #pragma unroll
@@ -241,7 +168,7 @@ __global__ void __launch_bounds__(kThreads) sampler_temperature_kernel(const Sam
     if (lane == 0) p.out[b] = best_id;
   }
   cluster.sync();  // keep every CTA's shared memory alive until rank 0 has read it
-  advance_rng(p);
+  advance_rng(p.rng_word);
 }
 
 // ===================================== full path ==================================================
@@ -326,31 +253,9 @@ __device__ void merge_lists(float* val, int* ids, float* tv, int* ti, int n) {
   }
 }
 
-__device__ __forceinline__ void online_add(float x, float& m, float& s) {
-  if (x == -INFINITY) return;
-  if (x > m) {
-    s = s * expf(m - x) + 1.f;
-    m = x;
-  } else {
-    s += expf(x - m);
-  }
-}
-
-__device__ __forceinline__ void online_merge(float m2, float s2, float& m, float& s) {
-  if (m2 == -INFINITY) return;
-  if (m == -INFINITY) {
-    m = m2, s = s2;
-  } else if (m2 > m) {
-    s = s * expf(m - m2) + s2;
-    m = m2;
-  } else {
-    s += s2 * expf(m2 - m);
-  }
-}
-
 template <typename T, int KMAX>
 __global__ void __launch_bounds__(kThreads, 1) sampler_full_kernel(const SamplerParams p) {
-  constexpr int kLists = kWarps > kMaxSlices ? kWarps : kMaxSlices;
+  constexpr int kLists = kWarps > kSamplerMaxSlices ? kWarps : kSamplerMaxSlices;
   __shared__ float lv[kLists * KMAX];
   __shared__ int li[kLists * KMAX];
   __shared__ float tv[kLists / 2 * KMAX];
@@ -361,7 +266,7 @@ __global__ void __launch_bounds__(kThreads, 1) sampler_full_kernel(const Sampler
   const int slice = static_cast<int>(cluster.block_rank());
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   pdl_wait();
-  const uint64_t offset = launch_offset(p);
+  const uint64_t offset = launch_offset(p.rng_word, p.rng_base);
   const T* row = static_cast<const T*>(p.logits) + b * p.row_stride;
   const RowScalars rs = row_scalars(p, b);
   const bool before = p.policy == 1;
@@ -426,7 +331,7 @@ __global__ void __launch_bounds__(kThreads, 1) sampler_full_kernel(const Sampler
   }
   cluster.sync();  // remote reads done: the other CTAs may leave
   if (slice != 0) {
-    advance_rng(p);
+    advance_rng(p.rng_word);
     return;
   }
   if (n > 1) merge_lists<KMAX>(lv, li, tv, ti, n);
@@ -500,46 +405,7 @@ __global__ void __launch_bounds__(kThreads, 1) sampler_full_kernel(const Sampler
       }
     }
   }
-  advance_rng(p);
-}
-
-// Smallest power-of-two slice count with slices * batch >= SMs, capped at the portable cluster
-// size 8 (so batches below 17 leave SMs idle), and no slice under 16 chunks.
-int pick_slices(int batch, int vocab) {
-  const int sms = sm_count() > 0 ? sm_count() : 132;
-  int s = 1;
-  while (s < kMaxSlices && s * batch < sms && vocab / 8 / (2 * s) >= 16) s *= 2;
-  return s;
-}
-
-struct RngState {
-  unsigned long long* word;
-  uint64_t base;
-};
-
-// Launch-offset word of `stream` (of its own for a captured launch); the base makes offsets of
-// different words disjoint, so two graphs or streams sampling with one seed draw different noise.
-int rng_state(cudaStream_t stream, RngState* st) {
-  uint64_t serial = 0;
-  int* w = stream_state(stream, &serial);
-  if (w == nullptr) return HPC_ERR_CUDA;
-  st->word = reinterpret_cast<unsigned long long*>(w);
-  st->base = serial << 40;
-  return HPC_OK;
-}
-
-int check_common(const void* logits, int64_t row_stride, int dtype, int batch, int vocab, int max_topk,
-                 const char* who) {
-  HPC_REQUIRE(dtype == 0 || dtype == 1, "%s: logits dtype must be float32 or bfloat16", who);
-  HPC_REQUIRE(batch >= 0 && batch <= 65535, "%s: batch %d out of range [0, 65535]", who, batch);
-  HPC_REQUIRE(vocab % 8 == 0 && vocab >= max_topk && vocab <= 262144,
-              "%s: vocab size %d must be a multiple of 8 in [%d, 262144]", who, vocab, max_topk);
-  const int elem = dtype == 0 ? 4 : 2;
-  HPC_REQUIRE(row_stride >= vocab && (row_stride * elem) % 16 == 0 &&
-                  reinterpret_cast<uintptr_t>(logits) % 16 == 0,
-              "%s: logits rows must be 16-byte aligned (row stride %lld elements)", who,
-              static_cast<long long>(row_stride));
-  return HPC_OK;
+  advance_rng(p.rng_word);
 }
 
 template <typename T>

@@ -100,8 +100,8 @@ lib.hpc_attention_blocksparse_prefill_qkpertoken_perhead_vperhead_fp8_async.argt
     _prefill_args + [c_i64] * 3 + [c_ptr])
 
 # (hasattr: a library built from an older commit, e.g. for an A/B timing, lacks these symbols; it
-# still fails loudly -- at the first rope, sampler, bf16 prefill, Stem, RMSNorm or masked
-# activation call)
+# still fails loudly -- at the first rope, sampler, speculative sampler, bf16 prefill, Stem, RMSNorm
+# or masked activation call)
 if hasattr(lib, "hpc_rope_norm_store_kv_async"):
     lib.hpc_rope_norm_store_kv_async.restype = c_int
     lib.hpc_rope_norm_store_kv_async.argtypes = [c_ptr] * 12 + [c_int] * 12 + [c_ptr]
@@ -125,6 +125,12 @@ if hasattr(lib, "hpc_fused_sampler_async"):
         [c_ptr, c_ptr, c_i64, c_int, c_int, c_int, c_ptr, c_f32, c_ptr, c_ptr, ctypes.c_uint64, c_ptr])
     lib.hpc_sampler_rng_offset.restype = c_int
     lib.hpc_sampler_rng_offset.argtypes = [c_ptr, ctypes.POINTER(ctypes.c_uint64)]
+
+if hasattr(lib, "hpc_fused_speculative_sampler_async"):
+    lib.hpc_fused_speculative_sampler_async.restype = c_int
+    lib.hpc_fused_speculative_sampler_async.argtypes = (
+        [c_ptr] * 4 + [c_i64] + [c_int] * 4 + [c_ptr, c_int, c_ptr, c_ptr, c_f32, c_ptr, c_ptr,
+                                              ctypes.c_uint64, c_ptr])
 
 if hasattr(lib, "hpc_stem_tpd_async"):
     lib.hpc_stem_oam_prep_paged_kv_qpertoken_perhead_kvpertensor_dim128_async.restype = c_int

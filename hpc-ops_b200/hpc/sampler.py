@@ -1,6 +1,8 @@
 """Fused token sampler (API of reference hpc/sampler.py): repetition penalty, temperature, optional
 softmax, top-k, top-p and Gumbel-max sampling of one token per row in one sm_90a kernel, and the
-penalty-mask write-back. No host synchronisation; capturable in a CUDA graph."""
+penalty-mask write-back. Fused speculative sampling (no reference counterpart): acceptance of
+multi-token-prediction drafts and the recovered or bonus token. No host synchronisation; capturable
+in a CUDA graph."""
 import ctypes
 from enum import IntEnum
 from typing import Optional, Tuple, Union
@@ -230,6 +232,115 @@ def fused_sampler(
     p, p_val = _per_row_arg(topp, "topp")
     return torch.ops.hpc.fused_sampler(logits, penalty_mask, slot_id, rp, rp_val, t, t_val, int(policy),
                                        k, k_val, p, p_val, max_topk, gumbel_noise, seed)
+
+
+_MAX_DRAFT = 8
+
+
+def _fused_speculative_sampler_impl(target_logits, draft_token_ids, draft_probs, temperature,
+                                    temperature_val, uniform=None, gumbel_noise=None, seed=0):
+    N, V, dtype = _check_logits(target_logits, 1)
+    dev = target_logits.device
+    _require(draft_token_ids.device == dev and draft_token_ids.dtype in (torch.int32, torch.int64)
+             and draft_token_ids.dim() == 2 and draft_token_ids.is_contiguous(),
+             "draft_token_ids must be a contiguous int32 or int64 [batch_size, K] tensor on the "
+             "device of target_logits")
+    B, K = draft_token_ids.shape
+    _require(1 <= K <= _MAX_DRAFT, f"K = {K} draft tokens per request; 1 to {_MAX_DRAFT} are supported")
+    _require(N == B * (K + 1), f"target_logits has {N} rows; batch_size {B} x (K + 1) = {B * (K + 1)} "
+             "expected (row b * (K + 1) + i is position i of request b)")
+    _require(N <= 65535, f"batch_size x (K + 1) = {N} rows exceeds 65535")
+    if draft_probs is not None:
+        _require(draft_probs.device == dev and draft_probs.dtype == torch.float32
+                 and draft_probs.is_contiguous() and tuple(draft_probs.shape) == (B, K, V)
+                 and draft_probs.data_ptr() % 16 == 0,
+                 f"draft_probs must be a contiguous, 16-byte aligned float32 [{B}, {K}, {V}] tensor "
+                 "on the device of target_logits")
+    _check_row_param(temperature, "temperature", B, (torch.float32,), dev)
+    _require((uniform is None) == (gumbel_noise is None),
+             "uniform and gumbel_noise go together: pass both or neither")
+    if uniform is None:
+        if temperature is not None or temperature_val > 0:
+            _require(seed > 0, f"sampling with the kernel's own noise needs a seed >= 1 (seed={seed}); "
+                     "pass uniform and gumbel_noise to sample without one")
+    else:
+        _require(uniform.device == dev and uniform.dtype == torch.float32 and uniform.is_contiguous()
+                 and tuple(uniform.shape) == (B, K),
+                 f"uniform must be a contiguous float32 [{B}, {K}] tensor on the device of target_logits")
+        _require(gumbel_noise.device == dev and gumbel_noise.dtype == torch.float32
+                 and gumbel_noise.is_contiguous() and tuple(gumbel_noise.shape) == (N, V)
+                 and gumbel_noise.data_ptr() % 16 == 0,
+                 f"gumbel_noise must be a contiguous, 16-byte aligned float32 [{N}, {V}] tensor on the "
+                 "device of target_logits")
+    out = torch.empty(B, K + 1, dtype=torch.int32, device=dev)
+    num_accepted = torch.empty(B, dtype=torch.int32, device=dev)
+    records = torch.empty(N, 8, dtype=torch.int32, device=dev)  # 32 bytes per row for the kernels
+    _check_rc(_lib.hpc_fused_speculative_sampler_async(
+        _ptr(out), _ptr(num_accepted), _ptr(records), _ptr(target_logits), target_logits.stride(0), dtype,
+        B, K, V, _ptr(draft_token_ids), int(draft_token_ids.dtype == torch.int64), _ptr(draft_probs),
+        _ptr(temperature), float(temperature_val), _ptr(uniform), _ptr(gumbel_noise), max(int(seed), 0),
+        _stream_of(target_logits)), "fused_speculative_sampler")
+    return out, num_accepted
+
+
+_ops.define("fused_speculative_sampler(Tensor target_logits, Tensor draft_token_ids, Tensor? draft_probs, "
+            "Tensor? temperature, float temperature_val, Tensor? uniform=None, Tensor? gumbel_noise=None, "
+            "int seed=0) -> (Tensor, Tensor)")
+_ops.impl("fused_speculative_sampler", _fused_speculative_sampler_impl, "CUDA")
+
+
+@torch.library.register_fake("hpc::fused_speculative_sampler")
+def _fused_speculative_sampler_fake(target_logits, draft_token_ids, draft_probs, temperature,
+                                    temperature_val, uniform=None, gumbel_noise=None, seed=0):
+    B, K = draft_token_ids.shape
+    return (target_logits.new_empty((B, K + 1), dtype=torch.int32),
+            target_logits.new_empty((B,), dtype=torch.int32))
+
+
+def fused_speculative_sampler(
+    target_logits: Tensor,
+    draft_token_ids: Tensor,
+    *,
+    draft_probs: Optional[Tensor] = None,
+    temperature: Union[Tensor, float] = 0.0,
+    uniform: Optional[Tensor] = None,
+    gumbel_noise: Optional[Tensor] = None,
+    seed: int = 0,
+) -> Tuple[Tensor, Tensor]:
+    """Verify K draft tokens per request against the target model and draw the next token.
+
+    `target_logits` [B * (K + 1), V] (float32 or bfloat16, rows 16-byte aligned, V % 8 == 0,
+    V <= 262144): row b * (K + 1) + i is position i of request b, the query order of
+    `attention_decode_*` with mtp = K. `draft_token_ids` [B, K] int32 or int64, 1 <= K <= 8.
+    Returns `output_token_ids` int32 [B, K + 1] and `num_accepted` int32 [B]: with
+    n = num_accepted[b] + 1, out[b, :n] holds the accepted drafts followed by the recovered or bonus
+    token, and out[b, n:] is -1. Every written id lies in [0, V).
+
+    With x = float(logits) and ties always going to the smaller token id, request b with
+    temperature t (a [B] float32 tensor or one scalar for every request):
+
+    * Greedy (t <= 0 or NaN): a_i = argmax x_i (a row without a non-NaN value gives 0). Draft d_i
+      is accepted while d_i == a_i; the first mismatch j emits a_j, and if all K are accepted a_K
+      is the bonus token. `draft_probs` is ignored.
+    * Sampling (t > 0): xt = x / t (IEEE division), p_i = softmax(xt_i), q_i = draft_probs[b, i]
+      ([B, K, V] float32, contiguous) or one-hot at d_i when it is None. d_i is accepted iff
+      0 <= d_i < V and u_i * q_i(d_i) < p_i(d_i). At the first rejection j the recovered token is,
+      for one-hot drafts, argmax over v != d_j of xt_j + g_j (exactly `fused_sampler` on that row
+      with `draft_token_ids=d_j`); with `draft_probs`, argmax over {v : p_j(v) > q_j(v)} of
+      log(p_j(v) - q_j(v)) + g_j(v), or argmax of xt_j + g_j when that set is empty. If all K are
+      accepted, the bonus token is argmax of xt_K + g_K. So the first emitted token is distributed
+      as p whenever the drafts were drawn from q.
+
+    `uniform` [B, K] and `gumbel_noise` [B * (K + 1), V] (float32, contiguous) make the result
+    deterministic and must be passed together. Without them the kernels draw Philox4x32-10 noise
+    keyed by `seed` (>= 1, needed whenever a request may sample) and the per-stream launch offset
+    that `fused_sampler` uses: g of token v in row r from counter (v / 4, r, offset) word v % 4,
+    u_{b,i} from counter (0xFFFFFFFF, b * (K + 1) + i, offset) word 0. Each such call advances the
+    offset by one, so successive calls and graph replays draw fresh noise.
+    """
+    t, t_val = _per_row_arg(temperature, "temperature")
+    return torch.ops.hpc.fused_speculative_sampler(target_logits, draft_token_ids, draft_probs, t,
+                                                   float(t_val), uniform, gumbel_noise, seed)
 
 
 def _rng_offset(device=None) -> int:

@@ -424,6 +424,27 @@ int hpc_fused_sampler_temperature_sample_async(
  * For tests: the internal noise of that launch is then known to the caller. */
 int hpc_sampler_rng_offset(cudaStream_t stream, uint64_t* offset);
 
+/* ---- fused speculative sampling ---------------------------------------------------------------
+ * No reference counterpart: verifies K draft tokens per request (multi-token prediction) against
+ * the target logits and draws the recovered or bonus token. target_logits [batch * (K + 1), vocab]
+ * fp32 (dtype 0) or bf16 (1), row b * (K + 1) + i = position i of request b, `row_stride` elements
+ * between rows, rows 16-byte aligned, vocab % 8 == 0, vocab <= 262144, 1 <= K = num_draft <= 8,
+ * batch * (K + 1) <= 65535. draft_token_ids [batch, K] int32 or int64 (draft_is_int64);
+ * draft_probs [batch, K, vocab] fp32 contiguous, 16-byte aligned, or null for one-hot drafts;
+ * temperature [batch] or, when null, temperature_val for every request (t <= 0 or NaN: greedy).
+ * uniform [batch, K] and gumbel_noise [batch * (K + 1), vocab] fp32 contiguous come together; when
+ * both are null a request with t > 0 draws Philox4x32-10 noise keyed by `seed` (>= 1) from the
+ * sampler's per-stream launch word, which the call then advances by one. Writes
+ * output_token_ids int32 [batch, K + 1] (accepted drafts, then the recovered or bonus token, then
+ * -1) and num_accepted int32 [batch]. row_records is a 16-byte aligned scratch of
+ * 32 * batch * (K + 1) bytes. Two launches chained by PDL, no allocation or host
+ * synchronisation: capturable. */
+int hpc_fused_speculative_sampler_async(
+    int* output_token_ids, int* num_accepted, void* row_records, const void* target_logits,
+    int64_t row_stride, int dtype, int batch, int num_draft, int vocab, const void* draft_token_ids,
+    int draft_is_int64, const float* draft_probs, const float* temperature, float temperature_val,
+    const float* uniform, const float* gumbel_noise, uint64_t seed, cudaStream_t stream);
+
 /* ---- Stem block-mask generation (block-sparse FP8 prefill) ----------------------------------
  * replaces reference src/stem/*.h, argument for argument (bool -> int), with cache and scale
  * strides added. Only stem_block_size 128, stem_stride 16 and head dim 128.

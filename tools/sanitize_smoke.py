@@ -1,6 +1,6 @@
 """One small invocation of every hot-path op (decode both quant types, prefill both, bf16 prefill
 dense and paged, blockwise + per-tensor MoE, route GEMM, W=1 allreduce, rope, the Stem mask stages,
-fused RMSNorm -> FP8 and the masked activation quantisers),
+fused RMSNorm -> FP8, the masked activation quantisers and the speculative sampler),
 meant to run under compute-sanitizer:
 
     compute-sanitizer --tool memcheck  python tools/sanitize_smoke.py
@@ -28,7 +28,7 @@ def cuda(d):
 
 def main():
     which = set(sys.argv[1:]) or {"decode", "prefill", "prefill_bf16", "moe", "gemm", "allreduce",
-                                  "rope", "stem", "norm_act"}
+                                  "rope", "stem", "norm_act", "spec"}
     if "decode" in which:
         B, hkv, hq = 3, 2, 8
         lens = [300, 129, 64]
@@ -161,6 +161,27 @@ def main():
                                     sent, scale=d["scale"])
             assert oact.masked_ok(res), res
         print("norm_act ok")
+    if "spec" in which:
+        import numpy as np
+        from oracle import spec_sampler as osp
+        from synth import spec_sampler as ssp
+        for probs in (False, True):  # given noise, then the kernel's own (checked for range only)
+            case = ssp.make_case(13, 6, 2, 4096, torch.bfloat16, probs=probs, pad=128)
+            n = case["np"]
+            dev = {k: torch.from_numpy(np.ascontiguousarray(n[k])).cuda() if n[k] is not None else None
+                   for k in ("draft_token_ids", "draft_probs", "temperature", "uniform", "noise")}
+            logits = case["store_t"].cuda()[:, :4096]
+            out, nacc = hpc.fused_speculative_sampler(
+                logits, dev["draft_token_ids"], draft_probs=dev["draft_probs"], temperature=dev["temperature"],
+                uniform=dev["uniform"], gumbel_noise=dev["noise"])
+            want, want_n = osp.spec_sample(n["store"], 4096, n["draft_token_ids"], draft_probs=n["draft_probs"],
+                                           temperature=n["temperature"], uniform=n["uniform"], noise=n["noise"])
+            assert np.array_equal(out.cpu().numpy(), want) and np.array_equal(nacc.cpu().numpy(), want_n)
+            out, nacc = hpc.fused_speculative_sampler(logits, dev["draft_token_ids"], draft_probs=dev["draft_probs"],
+                                                      temperature=dev["temperature"], seed=3)
+            o = out.cpu().numpy()
+            assert ((o >= 0) & (o < 4096) | (o == -1)).all()
+        print("spec ok")
     torch.cuda.synchronize()
     print("smoke ok")
 
