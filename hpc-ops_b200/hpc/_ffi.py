@@ -4,6 +4,7 @@ The library is the product: if `_C.so` is missing or a launcher reports an error
 raises — there is no CPU or PyTorch fallback anywhere in `hpc`.
 """
 import ctypes
+import re
 from pathlib import Path
 
 import torch
@@ -16,156 +17,74 @@ if len(_so_files) != 1:
         f"hpc (H100 build): expected exactly one _C*.so next to {__file__}, found "
         f"{len(_so_files)}. Build it with `python hpc-ops_b200/build.py` (needs nvcc, sm_90a)."
     )
-lib = ctypes.CDLL(str(_so_files[0]))
 
-c_int = ctypes.c_int
-c_i64 = ctypes.c_int64
-c_u32 = ctypes.c_uint32
-c_f32 = ctypes.c_float
-c_ptr = ctypes.c_void_p
+_HEADER = Path(__file__).resolve().parents[2] / "include" / "hpc_b200.h"
 
-lib.hpc_last_error.restype = ctypes.c_char_p
-lib.hpc_version.restype = ctypes.c_char_p
-lib.hpc_built_json.restype = ctypes.c_char_p
-lib.hpc_sm_count.restype = c_int
-
-lib.hpc_assign_attention_decode_task_host_bytes.restype = c_i64
-lib.hpc_assign_attention_decode_task_host_bytes.argtypes = [c_ptr] + [c_int] * 7
-lib.hpc_assign_attention_decode_task_sync.restype = c_int
-lib.hpc_assign_attention_decode_task_sync.argtypes = [c_ptr] + [c_int] * 7 + [c_ptr, c_i64]
-lib.hpc_assign_attention_decode_task_async.restype = c_int
-lib.hpc_assign_attention_decode_task_async.argtypes = [c_ptr, c_ptr] + [c_int] * 7 + [c_ptr]
-
-lib.hpc_attention_decode_fp8_async.restype = c_int
-lib.hpc_attention_decode_fp8_async.argtypes = (
-    [c_ptr] * 13 + [c_int] * 18 + [c_i64] * 6 + [c_ptr]
-)
-
-lib.hpc_attention_decode_bf16_async.restype = c_int
-lib.hpc_attention_decode_bf16_async.argtypes = [c_ptr] * 10 + [c_int] * 14 + [c_i64] * 6 + [c_ptr]
-
-for _n in ("hpc_attention_decode_fp8_partial_async", "hpc_attention_decode_fp8_combine_async"):
-    getattr(lib, _n).restype = c_int
-    getattr(lib, _n).argtypes = lib.hpc_attention_decode_fp8_async.argtypes
-
-lib.hpc_group_gemm_blockwise_fp8_async.restype = c_int
-lib.hpc_group_gemm_blockwise_fp8_async.argtypes = [c_ptr] * 11 + [c_int] * 10 + [c_ptr]
-lib.hpc_group_gemm_fp8_async.restype = c_int
-lib.hpc_group_gemm_fp8_async.argtypes = [c_ptr] * 10 + [c_int] * 8 + [c_ptr]
-lib.hpc_group_gemm_fp8_multistage_async.restype = c_int
-lib.hpc_group_gemm_fp8_multistage_async.argtypes = [c_ptr] * 9 + [c_int] * 7 + [c_ptr]
-lib.hpc_group_gemm_fp8_scatter_async.restype = c_int
-lib.hpc_group_gemm_fp8_scatter_async.argtypes = [c_ptr] * 10 + [c_int] * 7 + [c_ptr, c_int, c_ptr]
-lib.hpc_act_mul_and_quant_async.restype = c_int
-lib.hpc_act_mul_and_quant_async.argtypes = [c_ptr] * 3 + [c_int] * 3 + [c_ptr]
-lib.hpc_scaled_fp8_quant_async.restype = c_int
-lib.hpc_scaled_fp8_quant_async.argtypes = [c_ptr] * 3 + [c_i64, c_int, c_ptr]
-lib.hpc_reformat_x_scale_async.restype = c_int
-lib.hpc_reformat_x_scale_async.argtypes = [c_ptr] * 4 + [c_int] * 4 + [c_ptr]
-lib.hpc_count_and_gather_async.restype = c_int
-lib.hpc_count_and_gather_async.argtypes = [c_ptr] * 15 + [c_int] * 7 + [c_ptr]
-lib.hpc_blockwise_count_and_gather_async.restype = c_int
-lib.hpc_blockwise_count_and_gather_async.argtypes = [c_ptr] * 17 + [c_int] * 9 + [c_ptr]
-lib.hpc_reduce_async.restype = c_int
-lib.hpc_reduce_async.argtypes = [c_ptr] * 5 + [c_int] * 5 + [c_ptr]
-lib.hpc_fuse_moe_async.restype = c_int
-lib.hpc_fuse_moe_async.argtypes = [c_ptr] * 23 + [c_int] * 10 + [c_ptr]
-lib.hpc_fuse_moe_blockwise_async.restype = c_int
-lib.hpc_fuse_moe_blockwise_async.argtypes = [c_ptr] * 25 + [c_int] * 12 + [c_ptr]
-
-lib.hpc_fuse_allreduce_rmsnorm_high_throughput_async.restype = c_int
-lib.hpc_fuse_allreduce_rmsnorm_high_throughput_async.argtypes = (
-    [c_ptr] * 8 + [c_i64] * 3 + [ctypes.c_double, c_int, c_int, c_ptr])
-lib.hpc_fuse_allreduce_rmsnorm_high_throughput_p2p_async.restype = c_int
-lib.hpc_fuse_allreduce_rmsnorm_high_throughput_p2p_async.argtypes = (
-    [c_ptr] * 10 + [c_i64] * 3 + [ctypes.c_double, c_int, c_int, c_ptr])
-lib.hpc_fuse_allreduce_rmsnorm_low_latency_async.restype = c_int
-lib.hpc_fuse_allreduce_rmsnorm_low_latency_async.argtypes = (
-    [c_int] * 4 + [c_ptr] * 4 + [c_int] * 2 + [c_ptr] * 3 + [ctypes.c_double] + [c_ptr] * 2 + [c_int, c_ptr])
-lib.hpc_fuse_allreduce_rmsnorm_low_latency_ex_async.restype = c_int
-lib.hpc_fuse_allreduce_rmsnorm_low_latency_ex_async.argtypes = (
-    [c_int] * 4 + [c_ptr] * 4 + [c_int] * 2 + [c_ptr] * 3 + [ctypes.c_double] + [c_ptr] * 2 + [c_int, c_int, c_ptr])
-
-lib.hpc_gemm_bf16xfp32_select_splitk.restype = c_int
-lib.hpc_gemm_bf16xfp32_select_splitk.argtypes = [c_int] * 4
-lib.hpc_gemm_bf16xfp32_async.restype = c_int
-lib.hpc_gemm_bf16xfp32_async.argtypes = [c_ptr] * 6 + [c_int] * 3 + [c_f32] + [c_int] * 5 + [c_ptr]
-
-_prefill_args = [c_ptr] * 11 + [c_int] * 14 + [c_i64] * 6
-lib.hpc_attention_blocksparse_prefill_qpertoken_perhead_kvpertensor_fp8_async.restype = c_int
-lib.hpc_attention_blocksparse_prefill_qpertoken_perhead_kvpertensor_fp8_async.argtypes = (
-    _prefill_args + [c_ptr])
-lib.hpc_attention_blocksparse_prefill_qkpertoken_perhead_vperhead_fp8_async.restype = c_int
-lib.hpc_attention_blocksparse_prefill_qkpertoken_perhead_vperhead_fp8_async.argtypes = (
-    _prefill_args + [c_i64] * 3 + [c_ptr])
-
-# (hasattr: a library built from an older commit, e.g. for an A/B timing, lacks these symbols; it
-# still fails loudly -- at the first rope, sampler, speculative sampler, bf16 prefill, Stem, RMSNorm
-# or masked activation call)
-if hasattr(lib, "hpc_rope_norm_store_kv_async"):
-    lib.hpc_rope_norm_store_kv_async.restype = c_int
-    lib.hpc_rope_norm_store_kv_async.argtypes = [c_ptr] * 12 + [c_int] * 12 + [c_ptr]
-    lib.hpc_rope_norm_store_kv_fp8_async.restype = c_int
-    lib.hpc_rope_norm_store_kv_fp8_async.argtypes = [c_ptr] * 17 + [c_f32] + [c_int] * 14 + [c_ptr]
-
-if hasattr(lib, "hpc_attention_prefill_bf16_async"):
-    lib.hpc_attention_prefill_bf16_async.restype = c_int
-    lib.hpc_attention_prefill_bf16_async.argtypes = [c_ptr] * 6 + [c_int] * 11 + [c_ptr]
-    lib.hpc_attention_with_kvcache_prefill_bf16_async.restype = c_int
-    lib.hpc_attention_with_kvcache_prefill_bf16_async.argtypes = (
-        [c_ptr] * 7 + [c_int] * 12 + [c_i64] * 6 + [c_ptr])
-
-if hasattr(lib, "hpc_fused_sampler_async"):
-    lib.hpc_fused_sampler_async.restype = c_int
-    lib.hpc_fused_sampler_async.argtypes = (
-        [c_ptr, c_ptr, c_i64, c_int, c_int, c_int, c_ptr, c_i64, c_ptr, c_ptr, c_f32, c_ptr, c_f32,
-         c_int, c_ptr, c_int, c_int, c_ptr, c_f32, c_int, c_ptr, ctypes.c_uint64, c_ptr])
-    lib.hpc_fused_sampler_temperature_sample_async.restype = c_int
-    lib.hpc_fused_sampler_temperature_sample_async.argtypes = (
-        [c_ptr, c_ptr, c_i64, c_int, c_int, c_int, c_ptr, c_f32, c_ptr, c_ptr, ctypes.c_uint64, c_ptr])
-    lib.hpc_sampler_rng_offset.restype = c_int
-    lib.hpc_sampler_rng_offset.argtypes = [c_ptr, ctypes.POINTER(ctypes.c_uint64)]
-
-if hasattr(lib, "hpc_fused_speculative_sampler_async"):
-    lib.hpc_fused_speculative_sampler_async.restype = c_int
-    lib.hpc_fused_speculative_sampler_async.argtypes = (
-        [c_ptr] * 4 + [c_i64] + [c_int] * 4 + [c_ptr, c_int, c_ptr, c_ptr, c_f32, c_ptr, c_ptr,
-                                              ctypes.c_uint64, c_ptr])
-
-if hasattr(lib, "hpc_stem_tpd_async"):
-    lib.hpc_stem_oam_prep_paged_kv_qpertoken_perhead_kvpertensor_dim128_async.restype = c_int
-    lib.hpc_stem_oam_prep_paged_kv_qpertoken_perhead_kvpertensor_dim128_async.argtypes = (
-        [c_ptr] * 8 + [c_int] * 9 + [c_f32, c_int, c_int] + [c_i64] * 6 + [c_ptr, c_ptr])
-    lib.hpc_stem_oam_prep_paged_kv_qkpertoken_perhead_vperhead_dim128_async.restype = c_int
-    lib.hpc_stem_oam_prep_paged_kv_qkpertoken_perhead_vperhead_dim128_async.argtypes = (
-        [c_ptr] * 8 + [c_int] * 10 + [c_f32, c_int, c_int] + [c_i64] * 9 + [c_ptr, c_ptr])
-    lib.hpc_stem_oam_prep_varlen_q_dim128_async.restype = c_int
-    lib.hpc_stem_oam_prep_varlen_q_dim128_async.argtypes = (
-        [c_ptr] * 5 + [c_int] * 6 + [c_i64] * 3 + [c_ptr])
-    lib.hpc_stem_oam_gemm_dim128_async.restype = c_int
-    lib.hpc_stem_oam_gemm_dim128_async.argtypes = [c_ptr] * 6 + [c_int] * 8 + [c_ptr]
-    lib.hpc_stem_tpd_async.restype = c_int
-    lib.hpc_stem_tpd_async.argtypes = (
-        [c_ptr] * 5 + [c_int] * 5 + [c_f32, c_int, c_int, c_f32, c_int, c_f32, c_int, c_ptr])
+# The C types include/hpc_b200.h may use. Anything else is an error, not a guess: a ctypes c_int
+# slot silently truncates a 64-bit stride or a pointer.
+_PARAM_TYPES = {"int": ctypes.c_int, "int64_t": ctypes.c_int64, "uint64_t": ctypes.c_uint64,
+                "float": ctypes.c_float, "double": ctypes.c_double,
+                "cudaStream_t": ctypes.c_void_p}
+_RETURN_TYPES = {"int": ctypes.c_int, "int64_t": ctypes.c_int64, "const char*": ctypes.c_char_p}
+_PROTOTYPE = re.compile(r"^[ \t]*([A-Za-z_][\w \t*]*?)\s*\b(hpc_\w+)\s*\(([^()]*)\)\s*;", re.M)
 
 
-if hasattr(lib, "hpc_fused_rmsnorm_with_scale_async"):
-    lib.hpc_fused_rmsnorm_with_scale_async.restype = c_int
-    lib.hpc_fused_rmsnorm_with_scale_async.argtypes = [c_ptr] * 6 + [c_f32] + [c_int] * 3 + [c_ptr]
-    lib.hpc_masked_act_mul_and_quant_async.restype = c_int
-    lib.hpc_masked_act_mul_and_quant_async.argtypes = [c_ptr] * 4 + [c_int] * 3 + [c_ptr]
-    lib.hpc_masked_act_mul_and_blockwise_quant_async.restype = c_int
-    lib.hpc_masked_act_mul_and_blockwise_quant_async.argtypes = [c_ptr] * 4 + [c_int] * 3 + [c_ptr]
+def _param_type(fn: str, param: str):
+    if "*" in param:
+        return ctypes.c_void_p
+    m = re.fullmatch(r"(\w+(?: \w+)*) \w+", param)
+    typ = m.group(1) if m else param
+    if typ not in _PARAM_TYPES:
+        raise ImportError(f"hpc_b200.h: {fn} has a parameter of type {typ!r}, which has no ctypes "
+                          f"binding (allowed: pointers, {', '.join(_PARAM_TYPES)})")
+    return _PARAM_TYPES[typ]
 
-if hasattr(lib, "hpc_moe_topk_gating_async"):
-    lib.hpc_moe_topk_gating_async.restype = c_int
-    lib.hpc_moe_topk_gating_async.argtypes = [c_ptr] * 4 + [c_int] * 8 + [c_i64, c_f32, c_ptr]
+
+def prototypes(header_text: str) -> dict:
+    """{name: (restype, argtypes)} for every `RET hpc_name(PARAMS);` in a C header's text."""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", header_text, flags=re.S)
+    protos = {}
+    for ret, name, params in _PROTOTYPE.findall(text):
+        ret = re.sub(r" ?\*", "*", " ".join(ret.split()))
+        if ret not in _RETURN_TYPES:
+            raise ImportError(f"hpc_b200.h: {name} returns {ret!r}, which has no ctypes binding "
+                              f"(allowed: {', '.join(_RETURN_TYPES)})")
+        params = " ".join(params.split())
+        argtypes = [] if params == "void" else [_param_type(name, p.strip())
+                                                for p in params.split(",")]
+        protos[name] = (_RETURN_TYPES[ret], argtypes)
+    return protos
+
+
+def bind(lib, header_text: str | None = None):
+    """Set restype and argtypes of every function include/hpc_b200.h (or `header_text`) declares
+    and `lib` exports, and return `lib`. A declared function the library lacks (one built from an
+    older commit, e.g. for an A/B timing) stays unbound and fails at its first call."""
+    if header_text is None:
+        header_text = _HEADER.read_text()
+    for name, (restype, argtypes) in prototypes(header_text).items():
+        try:
+            fn = getattr(lib, name)
+        except AttributeError:
+            continue
+        fn.restype, fn.argtypes = restype, argtypes
+    return lib
+
+
+lib = bind(ctypes.CDLL(str(_so_files[0])))
+
 
 def check(rc: int, what: str = ""):
     """Turn a launcher status into the RuntimeError the reference raises via TORCH_CHECK."""
     if rc != 0:
         msg = lib.hpc_last_error().decode("utf-8", "replace")
         raise RuntimeError(f"hpc {what} failed (code {rc}): {msg}")
+
+
+def require(cond: bool, msg: str):
+    """Reject an argument the way a launcher would: RuntimeError, as the reference's TORCH_CHECK."""
+    if not cond:
+        raise RuntimeError(msg)
 
 
 def ptr(t):

@@ -4,7 +4,8 @@ from typing import Any as _Any, Optional as _Optional, Sequence as _Sequence, Tu
 import torch
 
 from . import _ops
-from ._ffi import check as _check_rc, lib as _lib, ptr as _ptr, stream_of as _stream_of
+from ._ffi import (check as _check_rc, lib as _lib, ptr as _ptr, require as _require,
+                   stream_of as _stream_of)
 from .communicator import MulticastCommunicator
 from .multicast_handle import MulticastHandle, _find_handle
 
@@ -13,11 +14,6 @@ import os as _os
 
 # world sizes up to which the high-throughput path prefers direct P2P loads/stores over NVLS
 _P2P_MAX_WORLD = int(_os.environ.get("HPC_B200_AR_P2P_MAX_WORLD", "2"))
-
-
-def _require(cond: bool, msg: str):
-    if not cond:
-        raise RuntimeError(msg)
 
 
 def _ht_impl(input, mc_input, in_residual, weight, signal, rank, world_size, num_max_blocks,

@@ -20,7 +20,8 @@ import torch
 from torch import Tensor
 
 from . import _ffi, _ops
-from ._ffi import check as _check_rc, lib as _lib, ptr as _ptr, stream_of as _stream_of
+from ._ffi import (check as _check_rc, lib as _lib, ptr as _ptr, require as _require,
+                   stream_of as _stream_of)
 
 
 class QuantType(_Enum):
@@ -49,11 +50,6 @@ def _num_total_ctas(device=None) -> int:
 # --------------------------------------------------------------------------------------------
 # torch.ops.hpc.* implementations
 # --------------------------------------------------------------------------------------------
-def _require(cond: bool, msg: str):
-    if not cond:
-        raise RuntimeError(msg)
-
-
 def _attention_decode_fp8_impl(
     q, kcache, vcache, block_ids, num_seq_kvcache, qscale, kscale, vscale, mtp, new_kv_included,
     quant_type, use_splitk, task_map, split_flag, output,

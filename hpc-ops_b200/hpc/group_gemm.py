@@ -5,12 +5,8 @@ import torch
 from torch import Tensor
 
 from . import _ops
-from ._ffi import check as _check_rc, lib as _lib, ptr as _ptr, stream_of as _stream_of
-
-
-def _require(cond: bool, msg: str):
-    if not cond:
-        raise RuntimeError(msg)
+from ._ffi import (check as _check_rc, lib as _lib, ptr as _ptr, require as _require,
+                   stream_of as _stream_of)
 
 
 def _scale_tile(avg: int) -> int:

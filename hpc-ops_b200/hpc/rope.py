@@ -5,14 +5,10 @@ import torch
 from torch import Tensor
 
 from . import _ops
-from ._ffi import check as _check_rc, lib as _lib, ptr as _ptr, stream_of as _stream_of
+from ._ffi import (check as _check_rc, lib as _lib, ptr as _ptr, require as _require,
+                   stream_of as _stream_of)
 
 _FP8_MAX = 448.0
-
-
-def _require(cond: bool, msg: str):
-    if not cond:
-        raise RuntimeError(msg)
 
 
 def _geometry(kcache, vcache, qkv, num_seqlen_per_req, kvcache_indices):

@@ -11,7 +11,8 @@ import torch
 from torch import Tensor
 
 from . import _ops
-from ._ffi import check as _check_rc, lib as _lib, ptr as _ptr, stream_of as _stream_of
+from ._ffi import (check as _check_rc, lib as _lib, ptr as _ptr, require as _require,
+                   stream_of as _stream_of)
 
 
 class SoftmaxPolicy(IntEnum):
@@ -30,11 +31,6 @@ class SoftmaxPolicy(IntEnum):
 
 
 _MAX_VOCAB = 262144
-
-
-def _require(cond: bool, msg: str):
-    if not cond:
-        raise RuntimeError(msg)
 
 
 def _per_row_arg(value, name: str):

@@ -14,17 +14,13 @@ import torch
 from torch import Tensor
 
 from . import _ops
-from ._ffi import check as _check_rc, lib as _lib, ptr as _ptr, stream_of as _stream_of
+from ._ffi import (check as _check_rc, lib as _lib, ptr as _ptr, require as _require,
+                   stream_of as _stream_of)
 from .attention import QuantType
 
 _BLOCK = 128
 _STRIDE = 16
 _MAX_KB = 32768
-
-
-def _require(cond: bool, msg: str):
-    if not cond:
-        raise RuntimeError(msg)
 
 
 def _check_geometry(who: str, stem_block_size: int, stem_stride: int):

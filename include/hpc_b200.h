@@ -12,6 +12,10 @@
  *
  * Nothing here falls back to the CPU: a launcher either enqueues sm_90a kernels on `stream`
  * or fails loudly.
+ *
+ * The Python package binds its ctypes argtypes from this file (hpc/_ffi.py `bind`), so a
+ * declaration may only use int, int64_t, uint64_t, float, double, pointers and cudaStream_t
+ * parameters, (void), and int, int64_t or const char* returns; anything else fails the CPU tests.
  */
 #ifndef INCLUDE_HPC_B200_H_
 #define INCLUDE_HPC_B200_H_

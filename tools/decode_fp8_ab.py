@@ -104,11 +104,9 @@ def sweep(base_so: Path, iters: int, reps: int):
     from hpc import attention as hatt
     from synth import decode as sd
 
-    base = ctypes.CDLL(str(base_so))
-    fb = base.hpc_attention_decode_fp8_partial_async
-    fb.restype = ctypes.c_int
-    fb.argtypes = _ffi.lib.hpc_attention_decode_fp8_async.argtypes
-    fns = {"base": fb, "new": _ffi.lib.hpc_attention_decode_fp8_partial_async}
+    base = _ffi.bind(ctypes.CDLL(str(base_so)))
+    fns = {"base": base.hpc_attention_decode_fp8_partial_async,
+           "new": _ffi.lib.hpc_attention_decode_fp8_partial_async}
     B, Sq, Hkv, Hq, S, MPL = 64, 1, 8, 32, 8192, 64
 
     rows = []

@@ -97,11 +97,7 @@ def main():
     if a.normal:
         libs = {"normal": Path(a.normal), **libs}
     for name, so in libs.items():
-        lib = ctypes.CDLL(str(so))
-        fn = lib.hpc_attention_decode_fp8_partial_async
-        fn.restype = ctypes.c_int
-        fn.argtypes = _ffi.lib.hpc_attention_decode_fp8_async.argtypes
-        fns[name] = fn
+        fns[name] = _ffi.bind(ctypes.CDLL(str(so))).hpc_attention_decode_fp8_partial_async
     for fn in fns.values():
         _ffi.check(fn(*args))
     runs = {k: [] for k in fns}
