@@ -61,6 +61,26 @@ def _attention_decode_fp8_impl(
     return y
 
 
+def _decode_output(output, q, rows, num_head_q):
+    """The decode output: a new [rows, num_head_q, 128] bf16 tensor, or the caller's `output`
+    once checked. The split-k combine stores 8 bytes per lane (the attention kernel's direct write
+    of an unsplit pair: 2) at y + row * y.stride(0) + head * 128, so rows may be strided (a view
+    into a wider buffer, e.g. a fused output) but must hold [num_head_q, 128] contiguously, and
+    the base and the row stride are kept 16-byte aligned."""
+    if output is None:
+        return torch.empty((rows, num_head_q, 128), dtype=torch.bfloat16, device=q.device)
+    _require(output.is_cuda and output.device == q.device, "output tensor must be cuda, on q's device")
+    _require(output.dtype == torch.bfloat16, "output dtype must be bfloat16")
+    _require(tuple(output.shape) == (rows, num_head_q, 128),
+             "output must have shape [num_batch * num_seq_q, num_head_q, 128]")
+    _require(output.stride(2) == 1 and output.stride(1) == 128
+             and (rows == 1 or output.stride(0) >= num_head_q * 128),
+             "output rows must be [num_head_q, 128] contiguous and must not overlap")
+    _require(output.data_ptr() % 16 == 0 and (rows == 1 or output.stride(0) % 8 == 0),
+             "output and its row stride must be 16-byte aligned")
+    return output
+
+
 def _decode_fp8_prepare(
     q, kcache, vcache, block_ids, num_seq_kvcache, qscale, kscale, vscale, mtp, new_kv_included,
     quant_type, use_splitk, task_map, split_flag, output,
@@ -111,11 +131,7 @@ def _decode_fp8_prepare(
         _require(kscale.stride(3) == 1 and kscale.data_ptr() % 4 == 0 and ks_unit >= 1, "bad kscale layout")
         _require(vscale.numel() == num_head_k, "vscale must hold one scale per kv head")
 
-    if output is not None:
-        y = output
-    else:
-        y = torch.empty((num_batch * num_seq_q, num_head_q, num_dim_v), dtype=torch.bfloat16,
-                        device=q.device)
+    y = _decode_output(output, q, num_batch * num_seq_q, num_head_q)
 
     num_total_ctas = _num_total_ctas(q.device)
     if task_map is None:
@@ -186,11 +202,7 @@ def _attention_decode_bf16_impl(
     _require(q.stride(2) == 1 and q.stride(1) == num_dim_qk, "q must be contiguous in (head, dim)")
     _require(kcache.stride(3) == 1 and vcache.stride(3) == 1, "kv cache innermost dim must be contiguous")
 
-    if output is not None:
-        y = output
-    else:
-        y = torch.empty((num_batch * num_seq_q, num_head_q, num_dim_v), dtype=torch.bfloat16,
-                        device=q.device)
+    y = _decode_output(output, q, num_batch * num_seq_q, num_head_q)
 
     num_total_ctas = _num_total_ctas(q.device)
     if task_map is None:

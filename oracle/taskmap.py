@@ -78,3 +78,17 @@ def assign_ref(lens, num_total_ctas, num_head_kv, num_seq_q, tilen, new_kv_inclu
     out = np.zeros(nbytes // 4, dtype=np.int32)
     r.ref_assign_attention_decode_task(*a, out.ctypes.data_as(ctypes.c_void_p), nbytes)
     return out.reshape(-1, 12)
+
+
+def pair_chunks(lens, num_total_ctas, num_head_kv, num_seq_q, min_process_len,
+                new_kv_included=True):
+    """Split-k chunks of every (request, kv head) pair of the decode schedule: {(b, h): [(first
+    key, keys), ...]} in chunk order. lens as the decode call receives them."""
+    tm = assign(lens, num_total_ctas, num_head_kv, num_seq_q, 128, new_kv_included,
+                min_process_len)
+    rows = tm[1:1 + int(tm[0, 0]) * int(tm[0, 1])]
+    out = {}
+    for h, b, c, st, n in rows[:, :5].tolist():
+        if h >= 0 and b >= 0:
+            out.setdefault((b, h), []).append((c, st, n))
+    return {k: [(st, n) for _, st, n in sorted(v)] for k, v in out.items()}

@@ -1,4 +1,5 @@
-"""Synthetic FP8 attention inputs whose outputs depend visibly on Q, K, the scales and the masks.
+"""Synthetic FP8 (and bf16 decode) attention inputs whose outputs depend visibly on Q, K, the
+scales and the masks.
 
 The plain builders (synth/decode.py, synth/prefill.py) draw scores with a standard deviation of
 about 0.005, so the softmax is uniform and the output is the mean of V whatever Q and K are.
@@ -52,8 +53,8 @@ def _quant_rows(x, code_max):
     return _e4m3(x / s[..., None]), s.float()
 
 
-def _place_pages(lens, gen, extra=4):
-    nblk = [(n + PAGE - 1) // PAGE for n in lens]
+def _place_pages(lens, gen, extra=4, page=PAGE):
+    nblk = [(n + page - 1) // page for n in lens]
     num_blocks = sum(nblk) + len(lens) + extra
     perm = torch.randperm(num_blocks, generator=gen)[:sum(nblk)].to(torch.int32)
     ids = torch.zeros(len(lens), max(nblk), dtype=torch.int32)
@@ -64,10 +65,15 @@ def _place_pages(lens, gen, extra=4):
     return ids, num_blocks
 
 
-def _needle_positions(n, sq, rows, gen):
-    """One distinct visible key per row; rows ordered (q head in group, MTP row)."""
-    cand = [0, 63, 64, 65, 127, 128, 129, n // 2 + 7]
-    if n % PAGE:
+def _needle_positions(n, sq, rows, gen, page=PAGE, front=None, rotate=0):
+    """One distinct visible key per row; rows ordered (q head in group, MTP row). Rows of the
+    first q head take the last visible key of their MTP row; the others take the keys of `front`,
+    then the page and tile edges rotated by `rotate`, then (without `front`) the middle of the
+    request, then the last token of a partial page."""
+    edges = [0, page - 1, page, page + 1, 127, 128, 129]
+    k = rotate % len(edges)
+    cand = (list(front) + edges[k:] + edges[:k]) if front is not None else edges + [n // 2 + 7]
+    if n % page:
         cand.append(n - 1)
     used, out = set(), []
     for r in range(rows):
@@ -204,6 +210,103 @@ def make_decode_exact_inputs(kind, lens, num_seq_q, num_head_kv, num_head_q, k_p
     else:
         out.update(k_scale=k_scale.to(dev))
     return out
+
+
+def _chunk_needles(chunks, page):
+    """Keys a needle should sit on for a pair split into `chunks` [(start, keys)]: the first key
+    of page 32 of the first chunk longer than 32 pages (the decode producer fetches page ids 32 at
+    a time) and a key inside a middle chunk."""
+    out = []
+    for st, n in chunks:
+        if n > 32 * page:
+            out.append(st + 32 * page)
+            break
+    if len(chunks) > 1:
+        st, n = chunks[len(chunks) // 2] if len(chunks) > 2 else chunks[1]
+        out.append(st + n // 2 + 1)
+    return out
+
+
+def make_decode_bf16_exact_inputs(kind, lens, num_seq_q, num_head_kv, num_head_q, page,
+                                  temperature=4.0, layout="NHD", chunks=None, seed=0,
+                                  device="cpu"):
+    """BF16 paged decode inputs in the format of synth.decode.make_decode_bf16_inputs, pages of
+    `page` tokens; lens include the num_seq_q new tokens. kind "peaked" (random scores of standard
+    deviation `temperature`) or "needle" (one Hadamard direction per (request, q head, MTP row),
+    and one key of the request holds it with score ln(len) + 3). Needles sit at the keys of
+    _needle_positions for this page size, at the last visible key of every MTP row and, given
+    `chunks` (oracle.taskmap.pair_chunks of the schedule the call will use), inside a middle
+    split-k chunk and on the first key of page 32 of a chunk longer than 32 pages. Poison (score
+    30) sits on each row's future MTP tokens, on every 8th key of a request for the next
+    request's rows, and, in both kinds, on the K slots past each request's length in its last
+    page. Their V slots are zero, as the API requires; poison goes in K only. The returned
+    "needles" maps (request, kv head) to the needle key of each row (rows ordered (q head in
+    group, MTP row))."""
+    gen = torch.Generator().manual_seed(seed)
+    lens = [int(n) for n in lens]
+    B, sq, hkv, hq = len(lens), num_seq_q, num_head_kv, num_head_q
+    g = hq // hkv
+    rows = g * sq
+    H = hadamard()
+    ids, nblocks = _place_pages(lens, gen, page=page)
+    qf = torch.zeros(B, sq, hq, D, dtype=torch.float64)
+    kf = torch.zeros(nblocks, page, hkv, D, dtype=torch.float64)
+    needles = {}
+    if kind == "peaked":
+        qf.normal_(generator=gen).mul_(temperature)
+        kf.normal_(generator=gen)
+    elif kind == "needle":
+        assert rows <= 32
+        kf.normal_(generator=gen)
+        for b, n in enumerate(lens):
+            dirs = H[(b % 4) * 32:(b % 4) * 32 + rows]
+            nxt = H[((b + 1) % 4) * 32:((b + 1) % 4) * 32 + rows].sum(0) if B > 1 else None
+            pg = ids[b, :(n + page - 1) // page].long()
+            for h in range(hkv):
+                kv = kf[pg, :, h].reshape(-1, D)  # this request's keys, a copy
+                for r in range(rows):
+                    gi, i = divmod(r, sq)
+                    qf[b, i, h * g + gi] = dirs[r]
+                front = _chunk_needles(chunks[(b, h)], page) if chunks is not None else None
+                pos = _needle_positions(n, sq, rows, gen, page, front, (b * hkv + h) * (rows - sq))
+                needles[(b, h)] = pos
+                for r in range(rows):
+                    gi, i = divmod(r, sq)
+                    kv[pos[r]] += (math.log(n) + 3.0) * dirs[r] / math.sqrt(D)
+                if nxt is not None and n > 3:
+                    other = torch.arange(3, n, 8)
+                    other = other[~torch.isin(other, torch.tensor(pos))]
+                    kv[other] += POISON * nxt / math.sqrt(D)
+                kf[pg, :, h] = kv.reshape(-1, page, D)
+    else:
+        raise ValueError(kind)
+    # future MTP tokens: key n - sq + j scores POISON for the rows i < j of its head group and
+    # nothing extra for the others (K through the pseudo-inverse of the group's query rows)
+    for b, n in enumerate(lens):
+        for h in range(hkv):
+            qg = qf[b, :, h * g:(h + 1) * g].transpose(0, 1).reshape(-1, D)  # rows (q head, MTP row)
+            mtp_row = torch.arange(rows) % sq
+            for j in range(1, min(sq, n)):
+                t = n - sq + j
+                want = POISON * math.sqrt(D) * (mtp_row < j).double()
+                kf[ids[b, t // page], t % page, h] += (torch.linalg.pinv(qg) @ want)
+    v = torch.randn(nblocks, page, hkv, D, generator=gen, dtype=torch.float64)
+    for b, n in enumerate(lens):
+        if n % page == 0:
+            continue
+        last = int(ids[b, (n + page - 1) // page - 1])
+        v[last, n % page:] = 0  # API contract: unused V slots are zero
+        for h in range(hkv):  # K slots past the length: score POISON for every row
+            qr = qf[b, :, h * g:(h + 1) * g].reshape(-1, D)
+            qr = qr / (qr * qr).sum(-1, keepdim=True)
+            kf[last, n % page:, h] += POISON * math.sqrt(D) * qr.sum(0)
+    kvcache = torch.stack([kf, v], 1).to(torch.bfloat16)
+    if layout == "HND":
+        kvcache = kvcache.permute(0, 1, 3, 2, 4).contiguous().permute(0, 1, 3, 2, 4)
+    dev = torch.device(device)
+    return dict(q=qf.reshape(B * sq, hq, D).to(torch.bfloat16).to(dev), kvcache=kvcache.to(dev),
+                block_ids=ids.to(dev), kv_lens_total=torch.tensor(lens, dtype=torch.int32, device=dev),
+                needles=needles)
 
 
 def make_prefill_exact_inputs(q_lens, kv_lens, num_head_q, num_head_kv, skip, k_per_token,

@@ -114,9 +114,29 @@ def test_decode_bf16_golden_fixtures(hpc):
         _check(_run(hpc, d, B, sq, hkv), torch.from_numpy(z["out"]), name)
 
 
+def _strided_q(q, extra_heads):
+    """q as the leading columns of a fused [rows, (Hq + extra) * 128] qkv buffer."""
+    rows, hq, d = q.shape
+    buf = torch.randn(rows, (hq + extra_heads) * d, device=q.device).to(q.dtype)
+    buf[:, :hq * d] = q.reshape(rows, -1)
+    v = buf[:, :hq * d].view(rows, hq, d)
+    assert v.stride(0) > hq * d
+    return v
+
+
+def _strided_output(like, extra, sentinel=7.0):
+    """An output view whose rows are `extra` elements wider than [Hq, 128]; the buffer is filled
+    with `sentinel`."""
+    rows, hq, d = like.shape
+    buf = torch.full((rows, hq * d + extra), sentinel, dtype=torch.bfloat16, device=like.device)
+    return buf, buf[:, :hq * d].view(rows, hq, d)
+
+
 def test_decode_bf16_entry_variants_agree(hpc):
     """No task map (scheduled inside the call), device-assigned map, CPU-assigned map, lengths
-    passed without the new tokens, caller-provided output: one result."""
+    passed without the new tokens, caller-provided output, q as a row-strided view of a fused qkv
+    buffer, output as a row-strided view (split-k combine and the direct write of unsplit pairs):
+    one result, and nothing written outside the output view."""
     d = oa.make_decode_bf16_inputs(16, 2, [777] * 16, 4, 32, block_size=32, seed=5, device="cuda")
     a = _run(hpc, d, 16, 2, 4, use_task_map=False)
     b = _run(hpc, d, 16, 2, 4, min_process_len=512)
@@ -125,9 +145,17 @@ def test_decode_bf16_entry_variants_agree(hpc):
     out = torch.empty_like(d["q"])
     f = _run(hpc, d, 16, 2, 4, min_process_len=512, output=out)
     assert f.data_ptr() == out.data_ptr()
-    for t in (b, c, e, f):
+    g = _run(hpc, dict(d, q=_strided_q(d["q"], 16)), 16, 2, 4, min_process_len=512)
+    for t in (b, c, e, f, g):
         assert torch.equal(a, t)
     _check(a, _oracle(d, 2), "variants")
+    # min_process_len 4096: bins of 32 tiles, so some pairs are split and some are not
+    base = _run(hpc, d, 16, 2, 4, min_process_len=4096)
+    for mpl, want in ((512, a), (4096, base)):
+        buf, view = _strided_output(d["q"], 128)
+        y = _run(hpc, d, 16, 2, 4, min_process_len=mpl, output=view)
+        assert y.data_ptr() == view.data_ptr() and torch.equal(y, want)
+        assert bool((buf[:, 32 * 128:] == 7.0).all()), "written outside the output view"
 
 
 def test_decode_bf16_paging_invariance(hpc):
@@ -155,3 +183,24 @@ def test_decode_bf16_rejects_bad_arguments(hpc):
         hpc.attention_decode_bf16(d["q"], k, v, d["block_ids"], d["kv_lens_total"], mtp=5)
     with pytest.raises(RuntimeError, match="blocksize"):
         hpc.attention_decode_bf16(d["q"], k[:, :8], v[:, :8], d["block_ids"], d["kv_lens_total"])
+    for bad, what in _bad_outputs(d["q"]):
+        with pytest.raises(RuntimeError, match="output"):
+            hpc.attention_decode_bf16(d["q"], k, v, d["block_ids"], d["kv_lens_total"], output=bad)
+        torch.cuda.synchronize()
+        assert bool((bad == 7).all()), f"{what}: written before the rejection"
+
+
+def _bad_outputs(q):
+    """Outputs both decode wrappers must reject before any launch, each filled with 7."""
+    rows, hq, d = q.shape
+    full = lambda *s, **kw: torch.full(s, 7, device=kw.get("device", "cuda"),  # noqa: E731
+                                       dtype=kw.get("dtype", torch.bfloat16))
+    return [
+        (full(rows, hq, d, dtype=torch.float32), "float32"),
+        (full(rows - 1, hq, d), "one row short"),
+        (full(rows, hq, d, device="cpu"), "on the CPU"),
+        (full(rows, hq, 2 * d)[:, :, :d], "head stride 256"),
+        (full(rows * hq * d).as_strided((rows, hq, d), (hq * d - d, d, 1)), "overlapping rows"),
+        (full(rows, hq * d + 16)[:, 4:4 + hq * d].view(rows, hq, d), "base not 16-byte aligned"),
+        (full(rows, hq * d + 4)[:, :hq * d].view(rows, hq, d), "row stride not 16-byte aligned"),
+    ]

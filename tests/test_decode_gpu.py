@@ -68,7 +68,7 @@ def test_taskmap_reassign_same_workspace(hpc):
 # decode attention
 # ------------------------------------------------------------------------------------------------
 def _run_decode(hpc, d, num_batch, num_seq_q, hkv, min_process_len=1024, use_task_map=True,
-                cpu_assign=False):
+                cpu_assign=False, output=None):
     lens = d["kv_lens_total"]
     task_map = None
     if use_task_map:
@@ -79,7 +79,7 @@ def _run_decode(hpc, d, num_batch, num_seq_q, hkv, min_process_len=1024, use_tas
         d["q"], d["kvcache"][:, 0], d["kvcache"][:, 1], d["block_ids"], lens, d["q_scale"],
         d["k_scale"], d["v_scale"], mtp=num_seq_q - 1, new_kv_included=True,
         quant_type=hpc.QuantType.QPERTOKEN_PERHEAD_KPERTENSOR_VPERTENSOR, splitk=True,
-        task_map=task_map)
+        task_map=task_map, output=output)
 
 
 def _check(my, gt, tag="", atol=0.2, rel_max=0.03):
@@ -156,11 +156,24 @@ def test_decode_fp8_golden_fixtures(hpc):
 
 
 def test_decode_fp8_without_task_map_and_cpu_assigned_map(hpc):
+    """Also: q as a row-strided view of a fused qkv buffer, and output as a row-strided view
+    (split-k combine and the direct write of unsplit pairs): the same bits, and nothing written
+    outside the output view."""
+    from test_decode_bf16_gpu import _strided_output, _strided_q
+
     d = oa.make_decode_fp8_inputs(16, 2, [777] * 16, 4, 32, seed=5, device="cuda")
     a = _run_decode(hpc, d, 16, 2, 4, use_task_map=False)
     b = _run_decode(hpc, d, 16, 2, 4, min_process_len=512)
     c = _run_decode(hpc, d, 16, 2, 4, min_process_len=512, cpu_assign=True)
     assert torch.equal(a, b) and torch.equal(b, c)
+    g = _run_decode(hpc, dict(d, q=_strided_q(d["q"], 16)), 16, 2, 4, min_process_len=512)
+    assert torch.equal(a, g)
+    base = _run_decode(hpc, d, 16, 2, 4, min_process_len=4096)  # some pairs split, some not
+    for mpl, want in ((512, a), (4096, base)):
+        buf, view = _strided_output(d["q"], 128)
+        y = _run_decode(hpc, d, 16, 2, 4, min_process_len=mpl, output=view)
+        assert y.data_ptr() == view.data_ptr() and torch.equal(y, want)
+        assert bool((buf[:, 32 * 128:] == 7.0).all()), "written outside the output view"
 
 
 def test_decode_fp8_paging_invariance_and_schedule_invariance(hpc):
@@ -285,3 +298,12 @@ def test_decode_rejects_unsupported(hpc):
         hpc.attention_decode_fp8(d["q"].float(), d["kvcache"][:, 0], d["kvcache"][:, 1],
                                  d["block_ids"], d["kv_lens_total"], d["q_scale"], d["k_scale"],
                                  d["v_scale"])
+    from test_decode_bf16_gpu import _bad_outputs
+
+    for bad, what in _bad_outputs(d["q"]):
+        with pytest.raises(RuntimeError, match="output"):
+            hpc.attention_decode_fp8(d["q"], d["kvcache"][:, 0], d["kvcache"][:, 1],
+                                     d["block_ids"], d["kv_lens_total"], d["q_scale"],
+                                     d["k_scale"], d["v_scale"], output=bad)
+        torch.cuda.synchronize()
+        assert bool((bad == 7).all()), f"{what}: written before the rejection"
