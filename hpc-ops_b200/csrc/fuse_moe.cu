@@ -431,3 +431,54 @@ extern "C" int hpc_fuse_moe_async(
                      static_cast<const float*>(topk_scale_ptr), shared_output_ptr, num_seq,
                      hidden_size, num_topk, stream);
 }
+
+// bf16 FusedMoE (no reference counterpart): route -> fused Gate-Up GEMM (SiLU*mul epilogue) ->
+// Down GEMM -> reduce, one PDL chain on `stream`, no allocation and no host synchronisation.
+// `intermediate_size` is I (gate_up_weight.size(1) / 2). Every limit is checked before the first
+// launch.
+extern "C" int hpc_fuse_moe_bf16_async(
+    void* output_ptr, const void* input_ptr, void* gate_up_input_ptr, const void* gate_up_weight_ptr,
+    void* down_input_ptr, void* down_output_ptr, const void* down_weight_ptr,
+    const void* topk_ids_ptr, const void* topk_scale_ptr, void* topk_pos_ptr, void* counts_ptr,
+    void* cu_counts_ptr, void* tiles_ptr, void* cu_tiles_ptr, const void* shared_output_ptr,
+    int num_tokens, int hidden_size, int intermediate_size, int num_topk, int num_expert_total,
+    int num_expert_local, int rank_ep, cudaStream_t stream) {
+  HPC_REQUIRE(num_tokens >= 0, "fuse_moe_bf16: negative num_tokens %d", num_tokens);
+  HPC_REQUIRE(num_expert_local > 0 && num_expert_local <= moe::kMaxExperts,
+              "fuse_moe_bf16: local experts %d not in (0, %d]", num_expert_local, moe::kMaxExperts);
+  HPC_REQUIRE(num_expert_total >= num_expert_local,
+              "fuse_moe_bf16: num_expert_total %d below the %d local experts", num_expert_total,
+              num_expert_local);
+  HPC_REQUIRE(num_topk > 0 && num_topk <= 128, "fuse_moe_bf16: num_topk %d not in (0, 128]", num_topk);
+  HPC_REQUIRE(hidden_size > 0 && hidden_size % 128 == 0,
+              "fuse_moe_bf16: hidden (%d) must be a positive multiple of 128", hidden_size);
+  HPC_REQUIRE(intermediate_size > 0 && intermediate_size % 128 == 0,
+              "fuse_moe_bf16: intermediate (%d) must be a positive multiple of 128", intermediate_size);
+  const void* ptrs[] = {output_ptr, input_ptr, gate_up_input_ptr, gate_up_weight_ptr, down_input_ptr,
+                        down_output_ptr, down_weight_ptr, shared_output_ptr};
+  for (const void* q : ptrs) {
+    HPC_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0, "fuse_moe_bf16: tensors must be 16-byte aligned");
+  }
+  if (num_tokens == 0) return HPC_OK;
+  const int rows = num_tokens * num_topk;
+  const int* counts = static_cast<const int*>(counts_ptr);
+  const int* cu_counts = static_cast<const int*>(cu_counts_ptr);
+  // a bf16 row is 2*H bytes for the route kernel's byte copy; the tile counts it writes are in
+  // 128-row m-tiles of the bf16 GEMM
+  int rc = moe::route(input_ptr, nullptr, gate_up_input_ptr, nullptr,
+                      static_cast<const int*>(topk_ids_ptr), static_cast<int*>(topk_pos_ptr),
+                      static_cast<int*>(counts_ptr), static_cast<int*>(cu_counts_ptr),
+                      static_cast<int*>(tiles_ptr), static_cast<int*>(cu_tiles_ptr), num_tokens,
+                      num_topk, 2 * hidden_size, num_expert_local, rank_ep, 128, 0, stream);
+  if (rc) return rc;
+  rc = ggemm::run_bf16(true, gate_up_input_ptr, gate_up_weight_ptr, counts, cu_counts,
+                       down_input_ptr, num_expert_local, rows, 2 * intermediate_size, hidden_size,
+                       stream);
+  if (rc) return rc;
+  rc = ggemm::run_bf16(false, down_input_ptr, down_weight_ptr, counts, cu_counts, down_output_ptr,
+                       num_expert_local, rows, hidden_size, intermediate_size, stream);
+  if (rc) return rc;
+  return moe::reduce(output_ptr, down_output_ptr, static_cast<const int*>(topk_pos_ptr),
+                     static_cast<const float*>(topk_scale_ptr), shared_output_ptr, num_tokens,
+                     hidden_size, num_topk, stream);
+}

@@ -29,6 +29,7 @@
 //               up values of one output column are in the same thread, the amax of a row over its
 //               128 quantised columns is a reduction over the 4 threads of a quad.
 #include "common.cuh"
+#include "group_gemm_sched.cuh"
 #include "host_utils.h"
 
 namespace b200 {
@@ -74,64 +75,12 @@ struct Params {
   int* tile_counter;  // dynamic tile scheduler: [0] next tile, [1] CTAs done (self-resetting)
 };
 
-__device__ __forceinline__ float silu_f(float x) {
-  // x / (1 + exp(-x)) with ex2.approx / approximate division (relative error ~1e-6, far below
-  // the bf16 / e4m3 granularity around it; reference src/utils/utils.cuh:300-330 does the same).
-  // An IEEE expf + division here costs ~35 % of a Gate-Up tile's MMA time in the epilogue.
-  return __fdividef(x, 1.f + __expf(-x));
-}
-
-__device__ __forceinline__ float bf16_round(float x) {
-  return __bfloat162float(__float2bfloat16_rn(x));
-}
-
-struct TileInfo {
-  int g, mt, nt;
-  int row0;    // first row (global) of the tile
-  int nvalid;  // valid rows in the tile
-  int scol0;   // first activation-scale column of the tile
-};
-
-// smem-resident schedule: cu_tiles (prefix of m-tiles*NT), pad_base (scale column base) per group
-struct Sched {
-  int* cu_tiles;   // [G+1]
-  int* pad_base;   // [G]
-  int* rows;       // [G]
-  int* row_start;  // [G]
-  int num_group;
-  int nt_count;
-};
-
 // dynamic shared memory: operand stages, fp16 operand copy, schedule arrays, scale rings, barriers,
 // tile queue
 constexpr int kSmemBytes = kStages * kStageBytes + kF16Bytes + (kMaxGroups + 4 + 3 * kMaxGroups) * 4 +
                            kXsSlots * kBM * 4 + kTileQ * 2 * kMaxKB * 4 +
                            (2 * kStages + 2 * kTileQ) * 8 + kTileQ * 4;
 static_assert(kSmemBytes <= 227 * 1024, "grouped GEMM smem exceeds the sm_90 per-block limit");
-
-__device__ __forceinline__ bool decode_tile(const Sched& s, int tile, TileInfo& t) {
-  if (tile >= s.cu_tiles[s.num_group]) return false;
-  int lo = 0, hi = s.num_group - 1;
-  while (lo < hi) {
-    int mid = (lo + hi + 1) >> 1;
-    if (s.cu_tiles[mid] <= tile) {
-      lo = mid;
-    } else {
-      hi = mid - 1;
-    }
-  }
-  const int g = lo;
-  const int local = tile - s.cu_tiles[g];
-  const int mtiles = (s.rows[g] + kBM - 1) / kBM;
-  t.g = g;
-  t.nt = local / mtiles;
-  t.mt = local - t.nt * mtiles;
-  t.row0 = s.row_start[g] + t.mt * kBM;
-  const int left = s.rows[g] - t.mt * kBM;
-  t.nvalid = left < kBM ? left : kBM;
-  t.scol0 = s.pad_base[g] + t.mt * kBM;
-  return true;
-}
 
 template <bool kBlockwise, bool kFused>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -180,32 +129,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   // ---- schedule prologue: every CTA derives the same tile list from seqlens ----
   if (warp == 2) {
     // one warp scans <= 512 groups
-    int carry_tiles = 0, carry_pad = 0;
-    for (int g0 = 0; g0 < p.num_group; g0 += 32) {
-      const int g = g0 + lane;
-      const int r = g < p.num_group ? p.seqlens[g] : 0;
-      const int mt = (r + kBM - 1) / kBM;
-      const int pd = (r + p.scale_tile - 1) / p.scale_tile * p.scale_tile;
-      int it = mt * nt_count, ip = pd;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int a = __shfl_up_sync(0xffffffffu, it, o);
-        const int b = __shfl_up_sync(0xffffffffu, ip, o);
-        if (lane >= o) {
-          it += a;
-          ip += b;
-        }
-      }
-      if (g < p.num_group) {
-        s_cu_tiles[g] = carry_tiles + it - mt * nt_count;
-        s_pad_base[g] = carry_pad + ip - pd;
-        s_rows[g] = r;
-        s_row_start[g] = p.cu_seqlens[g];
-      }
-      carry_tiles += __shfl_sync(0xffffffffu, it, 31);
-      carry_pad += __shfl_sync(0xffffffffu, ip, 31);
-    }
-    if (lane == 0) s_cu_tiles[p.num_group] = carry_tiles;
+    GGEMM_SCHEDULE_SCAN(p, kBM, nt_count, s_cu_tiles, s_pad_base, s_rows, s_row_start, lane);
   }
   __syncthreads();
 
@@ -229,15 +153,10 @@ __global__ void __launch_bounds__(kThreads, 1)
       // Dynamic scheduler: tiles are claimed from a global counter, so tiles with neighbouring ids
       // (the m-tiles sharing one weight tile) start within a short window on different CTAs and
       // share that weight tile through L2. The id of the next tile is claimed one tile ahead.
-      auto claim = [&]() -> int {
-        int v = 0;
-        if (lane == 0) v = atomicAdd(p.tile_counter, 1);
-        return __shfl_sync(0xffffffffu, v, 0);
-      };
-      int next_tile = claim();
+      int next_tile = claim_tile(p.tile_counter, lane);
       while (true) {
         const int tile = next_tile;
-        bool valid = decode_tile(sched, tile, t);
+        bool valid = decode_tile<kBM>(sched, tile, t);
         valid = __shfl_sync(0xffffffffu, static_cast<int>(valid), 0) != 0;
         t.g = __shfl_sync(0xffffffffu, t.g, 0);
         t.nt = __shfl_sync(0xffffffffu, t.nt, 0);
@@ -265,7 +184,7 @@ __global__ void __launch_bounds__(kThreads, 1)
         __syncwarp();
         tq++;
         if (!valid) break;
-        next_tile = claim();
+        next_tile = claim_tile(p.tile_counter, lane);
         const int nrow0 = kFused ? t.nt * 128 : t.nt * kBN;
         const int nrow1 = kFused ? p.n / 2 + t.nt * 128 : t.nt * kBN + 128;
         // activation scales of the tile's rows: 16-byte granules covering the valid rows
@@ -298,16 +217,7 @@ __global__ void __launch_bounds__(kThreads, 1)
           __syncwarp();
         }
       }
-      // the last CTA out re-arms the scheduler for the next launch (no memset between launches:
-      // a memset node would break a PDL chain, and a graph replay needs nothing else)
-      if (lane == 0) {
-        __threadfence();
-        if (atomicAdd(p.tile_counter + 1, 1) == static_cast<int>(gridDim.x) - 1) {
-          p.tile_counter[0] = 0;
-          p.tile_counter[1] = 0;
-          __threadfence();
-        }
-      }
+      if (lane == 0) release_scheduler(p.tile_counter);
     }
   } else {
     // =========================== consumer warpgroups: wgmma + epilogue ====================
@@ -331,7 +241,7 @@ __global__ void __launch_bounds__(kThreads, 1)
         if (lane == 0) mbar_arrive(&tq_empty[qs]);
         break;
       }
-      decode_tile(sched, tile, t);
+      decode_tile<kBM>(sched, tile, t);
 
       // acc[h * 64 + i]: 128-column half h, register i of the m64n128 fragment (the m64n256
       // fragment has the same order: its columns 128..255 are registers 64..127)

@@ -5,7 +5,8 @@ scratch allocation — except that the bf16 Gate-Up scratch is not allocated: th
 SiLU*mul + FP8 re-quant into the Gate-Up GEMM epilogue.
 
 `moe_topk_gating` (no reference counterpart) turns the route GEMM's logits into the topk_ids /
-topk_scale these operators consume.
+topk_scale these operators consume, and `fuse_moe_bf16` (no reference counterpart either) runs the
+expert layer of a bf16 model.
 """
 from enum import IntEnum
 from typing import Optional
@@ -325,6 +326,144 @@ def _fuse_moe_blockwise_fp8_fake(x, x_scale, gate_up_weight, gate_up_weight_scal
 @torch.library.register_fake("hpc::reduce")
 def _reduce_fake(x, topk_pos, topk_scale, shared_output):
     return torch.empty((topk_pos.shape[0], x.shape[1]), dtype=torch.bfloat16, device=x.device)
+
+
+MAX_MOE_EXPERTS = 512
+MAX_MOE_TOPK = 128
+
+
+def _check_bf16(x, gate_up_weight, down_weight, topk_ids, topk_scale, num_expert_total,
+                shared_output, output):
+    """fuse_moe_bf16's limits, checked before any device work; returns (T, H, I, E_local, k)."""
+    for t, name, dt in ((x, "x", torch.bfloat16), (gate_up_weight, "gate_up_weight", torch.bfloat16),
+                        (down_weight, "down_weight", torch.bfloat16),
+                        (topk_ids, "topk_ids", torch.int32), (topk_scale, "topk_scale", torch.float32)):
+        _require(t.dtype == dt, f"fuse_moe_bf16: {name} must be {dt}, got {t.dtype}")
+        _require(t.is_contiguous(), f"fuse_moe_bf16: {name} must be contiguous")
+    _require(x.dim() == 2 and gate_up_weight.dim() == 3 and down_weight.dim() == 3
+             and topk_ids.dim() == 2,
+             "fuse_moe_bf16: x [T, H], gate_up_weight [E, 2I, H], down_weight [E, H, I] and "
+             "topk_ids [T, k] have the wrong number of dimensions")
+    T, H = x.shape
+    E, I2, H2 = gate_up_weight.shape
+    I = I2 // 2
+    _require(H % 128 == 0 and H > 0, f"fuse_moe_bf16: hidden {H} must be a positive multiple of 128")
+    _require(H2 == H, f"fuse_moe_bf16: gate_up_weight hidden {H2} differs from x's {H}")
+    _require(I2 % 256 == 0 and I2 > 0,
+             f"fuse_moe_bf16: gate_up_weight rows {I2} must be 2 * I with I a positive multiple of 128")
+    _require(tuple(down_weight.shape) == (E, H, I),
+             f"fuse_moe_bf16: down_weight must be [{E}, {H}, {I}], got {tuple(down_weight.shape)}")
+    _require(1 <= E <= MAX_MOE_EXPERTS,
+             f"fuse_moe_bf16: local experts {E} not in [1, {MAX_MOE_EXPERTS}]")
+    _require(num_expert_total >= E,
+             f"fuse_moe_bf16: num_expert_total {num_expert_total} below the {E} local experts")
+    _require(topk_ids.size(0) == T and tuple(topk_scale.shape) == tuple(topk_ids.shape),
+             f"fuse_moe_bf16: topk_ids and topk_scale must be [{T}, k]")
+    k = topk_ids.size(1)
+    _require(1 <= k <= MAX_MOE_TOPK, f"fuse_moe_bf16: num_topk {k} not in [1, {MAX_MOE_TOPK}]")
+    for t, name in ((shared_output, "shared_output"), (output, "output")):
+        if t is not None:
+            _require(t.dtype == torch.bfloat16 and tuple(t.shape) == (T, H) and t.is_contiguous(),
+                     f"fuse_moe_bf16: {name} must be a contiguous bf16 tensor of shape [{T}, {H}]")
+    for t, name in ((x, "x"), (gate_up_weight, "gate_up_weight"), (down_weight, "down_weight"),
+                    (topk_ids, "topk_ids"), (topk_scale, "topk_scale"),
+                    (shared_output, "shared_output"), (output, "output")):
+        _require(t is None or t.is_cuda, f"fuse_moe_bf16: {name} must be a CUDA tensor")
+        _require(t is None or t.device == x.device, f"fuse_moe_bf16: {name} must be on x's device")
+        _require(t is None or t.data_ptr() % 16 == 0, f"fuse_moe_bf16: {name} must be 16-byte aligned")
+    return T, H, I, E, k
+
+
+def _bf16_scratch(x, gate_up_weight, topk_ids):
+    """Intermediate tensors of the bf16 pipeline, by stage:
+      route    gate_up_input [rows, H] (gathered x rows, expert-major, token order inside an
+               expert), topk_pos [T, k], counts [E], cu_counts [E+1], tiles [E] (128-row m-tiles
+               per expert), cu_tiles [E+1];
+      Gate-Up  down_input [rows, I] bf16 (silu(g) * u);
+      Down     down_output [rows, H] bf16.
+    rows = T * k (an upper bound: ids of other ranks take no row)."""
+    num_tokens, hidden = x.shape
+    num_experts = gate_up_weight.size(0)
+    inter = gate_up_weight.size(1) // 2
+    num_topk = topk_ids.size(1)
+    rows = num_tokens * num_topk
+    dev = x.device
+    i32 = dict(dtype=torch.int32, device=dev)
+    return dict(
+        gate_up_input=torch.empty((rows, hidden), dtype=torch.bfloat16, device=dev),
+        down_input=torch.empty((rows, inter), dtype=torch.bfloat16, device=dev),
+        down_output=torch.empty((rows, hidden), dtype=torch.bfloat16, device=dev),
+        topk_pos=torch.empty((num_tokens, num_topk), **i32),
+        counts=torch.empty((num_experts,), **i32),
+        cu_counts=torch.empty((num_experts + 1,), **i32),
+        tiles=torch.empty((num_experts,), **i32),
+        cu_tiles=torch.empty((num_experts + 1,), **i32))
+
+
+def _launch_bf16(y, x, gate_up_weight, down_weight, topk_ids, topk_scale, shared_output, rank_ep,
+                 num_expert_total, s):
+    """Enqueue the whole bf16 pipeline with the scratch `s` of _bf16_scratch."""
+    num_tokens, hidden = x.shape
+    _check_rc(_lib.hpc_fuse_moe_bf16_async(
+        _ptr(y), _ptr(x), _ptr(s["gate_up_input"]), _ptr(gate_up_weight), _ptr(s["down_input"]),
+        _ptr(s["down_output"]), _ptr(down_weight), _ptr(topk_ids), _ptr(topk_scale),
+        _ptr(s["topk_pos"]), _ptr(s["counts"]), _ptr(s["cu_counts"]), _ptr(s["tiles"]),
+        _ptr(s["cu_tiles"]), _ptr(shared_output), num_tokens, hidden, gate_up_weight.size(1) // 2,
+        topk_ids.size(1), int(num_expert_total), gate_up_weight.size(0), int(rank_ep),
+        _stream_of(x)), "fuse_moe_bf16")
+
+
+def _fuse_moe_bf16_impl(x, gate_up_weight, down_weight, topk_ids, topk_scale, rank_ep,
+                        num_expert_total, shared_output, output):
+    T, H, _, _, _ = _check_bf16(x, gate_up_weight, down_weight, topk_ids, topk_scale,
+                                num_expert_total, shared_output, output)
+    y = output if output is not None else torch.empty((T, H), dtype=torch.bfloat16, device=x.device)
+    if T == 0:
+        return y
+    s = _bf16_scratch(x, gate_up_weight, topk_ids)
+    _launch_bf16(y, x, gate_up_weight, down_weight, topk_ids, topk_scale, shared_output, rank_ep,
+                 num_expert_total, s)
+    return y
+
+
+_ops.define(
+    "fuse_moe_bf16(Tensor x, Tensor gate_up_weight, Tensor down_weight, Tensor topk_ids, Tensor "
+    "topk_scale, int rank_ep, int num_expert_total, Tensor? shared_output, Tensor? output) -> "
+    "(Tensor)")
+_ops.impl("fuse_moe_bf16", _fuse_moe_bf16_impl, "CUDA")
+
+
+def fuse_moe_bf16(x: Tensor, gate_up_weight: Tensor, down_weight: Tensor, topk_ids: Tensor,
+                  topk_scale: Tensor, rank_ep: int, num_expert_total: int,
+                  shared_output: Optional[Tensor] = None, output: Optional[Tensor] = None) -> Tensor:
+    """bf16 FusedMoE: the expert layer of a bf16 MoE model in four sm_90a kernels (route, fused
+    Gate-Up GEMM + SiLU*mul, Down GEMM, top-k reduce) on the current stream.
+
+    x [T, H] bf16; gate_up_weight [E_local, 2I, H] bf16 (gate rows, then up rows, as fuse_moe* and
+    vLLM's w13); down_weight [E_local, H, I] bf16; topk_ids int32 / topk_scale float32 [T, k] as
+    moe_topk_gating returns them. This rank owns experts [rank_ep E_local, (rank_ep+1) E_local) of
+    num_expert_total; other ids contribute nothing. Per routed row r of local expert e, with fp32
+    accumulation:
+      1. g_j = bf16(sum_h x[h] W13[e, j, h]), u_j = bf16(sum_h x[h] W13[e, I+j, h]);
+      2. a_j = bf16(silu(g_j) * u_j), the product in fp32 (silu x / (1 + exp(-x)) with fast
+         exp and division, as the FP8 epilogue);
+      3. d = bf16(sum_j a_j W2[e, :, j]);
+      4. y[t] = bf16(sum_k topk_scale[t, k] d[pos[t, k]] (+ shared_output[t])), fp32 sums in k order.
+    Rows inside an expert are in token order, so two calls give the same bits.
+
+    Limits: H and I multiples of 128, 1 <= E_local <= 512, 1 <= k <= 128, contiguous 16-byte
+    aligned tensors on one device; otherwise RuntimeError before any launch. T = 0 returns without a
+    launch. shared_output [T, H] bf16 is added in the reduce; a caller-given output [T, H] bf16 is
+    written and returned. Scratch is allocated by torch's caching allocator, the launcher neither
+    allocates nor synchronises with the host: the call can be captured in a CUDA graph."""
+    return torch.ops.hpc.fuse_moe_bf16(x, gate_up_weight, down_weight, topk_ids, topk_scale,
+                                       int(rank_ep), int(num_expert_total), shared_output, output)
+
+
+@torch.library.register_fake("hpc::fuse_moe_bf16")
+def _fuse_moe_bf16_fake(x, gate_up_weight, down_weight, topk_ids, topk_scale, rank_ep,
+                        num_expert_total, shared_output, output):
+    return _moe_fake(x, output)
 
 
 class GatingScore(IntEnum):

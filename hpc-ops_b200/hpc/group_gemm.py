@@ -1,4 +1,5 @@
-"""Grouped FP8 GEMM operators (API of reference hpc/group_gemm.py)."""
+"""Grouped FP8 GEMM operators (API of reference hpc/group_gemm.py) and the grouped bf16 GEMM of
+fuse_moe_bf16 (no reference counterpart)."""
 from typing import Optional as _Optional
 
 import torch
@@ -229,3 +230,60 @@ def _group_gemm_fp8_scatter_cp_async_fake(x, weight, y_scale, row_indices, seqle
                                           tiles, cu_tiles, use_task_map=False):
     return torch.empty((row_indices.shape[0], weight.shape[1]), dtype=torch.bfloat16,
                        device=x.device)
+
+
+def _group_gemm_bf16_impl(x, weight, seqlens, cu_seqlens, output):
+    for tt, name, dt in ((x, "x", torch.bfloat16), (weight, "weight", torch.bfloat16),
+                         (seqlens, "seqlens", torch.int32), (cu_seqlens, "cu_seqlens", torch.int32)):
+        _require(tt.dtype == dt, f"group_gemm_bf16: {name} must be {dt}, got {tt.dtype}")
+        _require(tt.is_contiguous(), f"group_gemm_bf16: {name} must be contiguous")
+    _require(x.dim() == 2 and weight.dim() == 3,
+             "group_gemm_bf16: x must be [M, K] and weight [G, N, K]")
+    m, k = x.shape
+    g, n, k2 = weight.shape
+    _require(k2 == k, f"group_gemm_bf16: weight K {k2} differs from x's {k}")
+    _require(k % 128 == 0 and k > 0, f"group_gemm_bf16: K {k} must be a positive multiple of 128")
+    _require(n % 128 == 0 and n > 0, f"group_gemm_bf16: N {n} must be a positive multiple of 128")
+    _require(1 <= g <= 512, f"group_gemm_bf16: groups {g} not in [1, 512]")
+    _require(tuple(seqlens.shape) == (g,) and tuple(cu_seqlens.shape) == (g + 1,),
+             f"group_gemm_bf16: seqlens must be [{g}] and cu_seqlens [{g + 1}]")
+    if output is not None:
+        _require(output.dtype == torch.bfloat16 and tuple(output.shape) == (m, n)
+                 and output.is_contiguous(),
+                 f"group_gemm_bf16: output must be a contiguous bf16 tensor of shape [{m}, {n}]")
+    for tt, name in ((x, "x"), (weight, "weight"), (seqlens, "seqlens"), (cu_seqlens, "cu_seqlens"),
+                     (output, "output")):
+        _require(tt is None or tt.is_cuda, f"group_gemm_bf16: {name} must be a CUDA tensor")
+        _require(tt is None or tt.data_ptr() % 16 == 0,
+                 f"group_gemm_bf16: {name} must be 16-byte aligned")
+    y = output if output is not None else torch.empty((m, n), dtype=torch.bfloat16, device=x.device)
+    if m == 0:
+        return y
+    _check_rc(_lib.hpc_group_gemm_bf16_async(_ptr(y), _ptr(x), _ptr(weight), _ptr(seqlens),
+                                             _ptr(cu_seqlens), g, m, n, k, _stream_of(x)),
+              "group_gemm_bf16")
+    return y
+
+
+_ops.define("group_gemm_bf16(Tensor x, Tensor weight, Tensor seqlens, Tensor cu_seqlens, Tensor? "
+            "output) -> (Tensor)")
+_ops.impl("group_gemm_bf16", _group_gemm_bf16_impl, "CUDA")
+
+
+def group_gemm_bf16(x: Tensor, weight: Tensor, seqlens: Tensor, cu_seqlens: Tensor,
+                    output: _Optional[Tensor] = None) -> Tensor:
+    """Grouped bf16 GEMM: Y[rows of g] = X[rows of g] . weight[g]^T in one persistent sm_90a kernel.
+
+    x [M, K] bf16 holds the rows of group g at cu_seqlens[g] .. cu_seqlens[g] + seqlens[g]
+    (seqlens int32 [G], cu_seqlens int32 [G+1], as group_gemm_pertensor_fp8); weight [G, N, K]
+    bf16. Y [M, N] bf16 = bf16_rn of the fp32-accumulated products; rows outside every group are
+    not written. K and N multiples of 128, 1 <= G <= 512, contiguous 16-byte aligned tensors;
+    otherwise RuntimeError before any launch. A caller-given output is written and returned. No
+    allocation beyond the output and no host synchronisation: capturable in a CUDA graph."""
+    return torch.ops.hpc.group_gemm_bf16(x, weight, seqlens, cu_seqlens, output)
+
+
+@torch.library.register_fake("hpc::group_gemm_bf16")
+def _group_gemm_bf16_fake(x, weight, seqlens, cu_seqlens, output):
+    return output if output is not None else torch.empty((x.shape[0], weight.shape[1]),
+                                                         dtype=torch.bfloat16, device=x.device)

@@ -272,6 +272,33 @@ int hpc_fuse_moe_blockwise_async(
     int num_expert_local, int gate_up_weight_scale_lastdim_pad4, int down_weight_scale_lastdim_pad4,
     int rank_ep, cudaStream_t stream);
 
+/* ---- bf16 FusedMoE and its grouped bf16 GEMM ----------------------------------------------------
+ * No reference counterpart. x [num_tokens, H] bf16, gate_up_weight [E_local, 2I, H] bf16 (gate
+ * rows, then up rows), down_weight [E_local, H, I] bf16 (intermediate_size = I), topk_ids int32 /
+ * topk_scale f32 [num_tokens, num_topk]; experts [rank_ep E_local, (rank_ep+1) E_local) are local,
+ * other ids contribute nothing. Scratch (rows = num_tokens * num_topk): gate_up_input [rows, H],
+ * down_input [rows, I] and down_output [rows, H] bf16, topk_pos int32 [num_tokens, num_topk],
+ * counts / tiles int32 [E_local], cu_counts / cu_tiles int32 [E_local + 1] (tiles in 128-row
+ * m-tiles). Per routed row: g, u = bf16(fp32 GEMM), a = bf16(silu(g) * u) (fp32 product), d =
+ * bf16(a . W2^T), output[t] = bf16(sum_k topk_scale * d (+ shared_output[t])) in k order. H and I
+ * multiples of 128, E_local <= 512, num_topk <= 128, 16-byte aligned tensors, checked before any
+ * launch; num_tokens = 0 launches nothing. Route -> Gate-Up -> Down -> reduce on `stream` as one
+ * PDL chain, no allocation or host synchronisation: capturable. */
+int hpc_fuse_moe_bf16_async(
+    void* output_ptr, const void* input_ptr, void* gate_up_input_ptr, const void* gate_up_weight_ptr,
+    void* down_input_ptr, void* down_output_ptr, const void* down_weight_ptr,
+    const void* topk_ids_ptr, const void* topk_scale_ptr, void* topk_pos_ptr, void* counts_ptr,
+    void* cu_counts_ptr, void* tiles_ptr, void* cu_tiles_ptr, const void* shared_output_ptr,
+    int num_tokens, int hidden_size, int intermediate_size, int num_topk, int num_expert_total,
+    int num_expert_local, int rank_ep, cudaStream_t stream);
+/* y [m, n] bf16 = x [m, k] bf16 . w[g]^T (w [num_group, n, k] bf16) for the rows of group g
+ * (seqlens / cu_seqlens int32 as hpc_group_gemm_fp8_async), fp32 accumulation; rows outside every
+ * group are not written. k and n multiples of 128, 0 < num_group <= 512, 16-byte aligned x, w, y.
+ * Persistent, PDL, capturable. */
+int hpc_group_gemm_bf16_async(void* y_ptr, const void* x_ptr, const void* w_ptr,
+                              const void* seqlens_ptr, const void* cu_seqlens_ptr, int num_group,
+                              int m, int n, int k, cudaStream_t stream);
+
 /* ---- fused AllReduce + residual + RMSNorm -------------------------------------------------------
  * High throughput: replaces reference src/allreduce/fuse_allreduce_rmsnorm_high_throughput.h:12-18
  * (same arguments). `signal_ptr`: device int64[world_size] of signal-pad addresses; `mc_*`: the

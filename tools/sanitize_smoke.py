@@ -1,5 +1,5 @@
 """One small invocation of every hot-path op (decode both quant types, prefill both, bf16 prefill
-dense and paged, blockwise + per-tensor MoE, route GEMM, W=1 allreduce, rope, the Stem mask stages,
+dense and paged, blockwise + per-tensor MoE, bf16 MoE, route GEMM, W=1 allreduce, rope, the Stem mask stages,
 fused RMSNorm -> FP8, the masked activation quantisers and the speculative sampler),
 meant to run under compute-sanitizer:
 
@@ -27,8 +27,8 @@ def cuda(d):
 
 
 def main():
-    which = set(sys.argv[1:]) or {"decode", "prefill", "prefill_bf16", "moe", "gemm", "allreduce",
-                                  "rope", "stem", "norm_act", "spec"}
+    which = set(sys.argv[1:]) or {"decode", "prefill", "prefill_bf16", "moe", "moe_bf16", "gemm",
+                                  "allreduce", "rope", "stem", "norm_act", "spec"}
     if "decode" in which:
         B, hkv, hq = 3, 2, 8
         lens = [300, 129, 64]
@@ -95,6 +95,18 @@ def main():
         err = (y.float().cpu() - gt.float()).abs()
         assert float((err > 0.01 + 0.01 * gt.float().abs()).float().mean()) < 1e-3
         print("moe ok")
+    if "moe_bf16" in which:
+        from oracle import moe_bf16 as ob
+        from synth.moe_bf16 import make_moe_bf16_inputs
+        d = make_moe_bf16_inputs(40, 2, 256, 256, 16, routing="other_rank", size_ep=2, rank_ep=1,
+                                 shared=True, seed=6)
+        c = cuda(d)
+        y = hpc.fuse_moe_bf16(c["x"], c["gate_up_weight"], c["down_weight"], c["topk_ids"],
+                              c["topk_scale"], 1, 16, shared_output=c["shared_output"])
+        gt = ob.reference_fp32(d["x"], d["gate_up_weight"], d["down_weight"], d["topk_ids"],
+                               d["topk_scale"], 1, 16, d["shared_output"])
+        torch.testing.assert_close(y.float().cpu(), gt.float(), atol=2e-2, rtol=2e-2)
+        print("moe_bf16 ok")
     if "gemm" in which:
         from oracle import gemm as og
         x, w, wh, wl, scale = og.make_inputs(48, 192, 1024, device="cuda")
