@@ -477,7 +477,13 @@ static int launch(bool fp8, const Params& p, cudaStream_t stream) {
   if (p.norm_policy != 0) {
     HPC_REQUIRE(p.q_norm_w != nullptr && p.k_norm_w != nullptr, "rope: norm weights required");
   }
-  if (p.num_rows <= 0) return HPC_OK;
+  if (p.num_rows <= 0) {
+    // no kernel runs, but the split-k flags are still returned zeroed
+    if (fp8 && p.split_k_flag != nullptr) {
+      HPC_CUDA_CHECK(cudaMemsetAsync(p.split_k_flag, 0, sizeof(int) * p.num_req * p.hkv, stream));
+    }
+    return HPC_OK;
+  }
   const bool aligned16 = ((reinterpret_cast<uintptr_t>(p.qkv) | reinterpret_cast<uintptr_t>(p.cos_sin) |
                            reinterpret_cast<uintptr_t>(p.out_q) | reinterpret_cast<uintptr_t>(p.kcache) |
                            reinterpret_cast<uintptr_t>(p.vcache) | reinterpret_cast<uintptr_t>(p.out_k) |

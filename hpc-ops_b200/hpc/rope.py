@@ -128,7 +128,11 @@ def rope_norm_store_kv(
     """NeoX RoPE on Q/K of the packed bf16 `qkv` rows, optional per-head RMSNorm (policy 1: after,
     2: before the rotation), K/V written into the paged bf16 cache (or into out_k / out_v), the
     unused tail of each request's last page zeroed. Returns the rotated Q [rows, Hq, D]
-    (contract of reference hpc/rope.py:8-105)."""
+    (contract of reference hpc/rope.py:8-105).
+
+    The call writes only the slots of its rows and, for a request with rows in the call, the
+    tail of the page of its last token. A request with no new rows leaves its pages untouched,
+    and with out_k / out_v given no cache byte is written at all (no tail is zeroed either)."""
     return torch.ops.hpc.rope_norm_store_kv(
         key_cache, value_cache, qkv, cos_sin, num_seqlen_per_req, q_index, kvcache_indices,
         is_prefill, q_norm_weight, k_norm_weight, out_q, out_k, out_v, qk_norm_policy)
@@ -158,7 +162,9 @@ def rope_norm_store_kv_fp8(
     static per-tensor scales (x / scale); Q is quantised per token and head with a dynamic scale
     amax / upper_max (quant_policy 1; scales returned as [num_req, Hq, pad128(max_seqlens)] in
     prefill and [rows, Hq] in decode) or with the caller's q_scale_inv (quant_policy 2, q_scale is
-    None). Returns (q_fp8, q_scale, split_k_flag[num_req, Hkv] zeroed)."""
+    None). Returns (q_fp8, q_scale, split_k_flag[num_req, Hkv] zeroed, also when there are no
+    rows). Cache writes follow rope_norm_store_kv: only the rows' slots and the last page's tail
+    of a request with rows; nothing with out_k / out_v."""
     return _rope_fp8_impl(key_cache, value_cache, qkv, cos_sin, num_seqlen_per_req, q_index,
                           kvcache_indices, is_prefill, k_scale, v_scale, int(quant_policy),
                           int(max_seqlens), upper_max, q_scale_inv, q_norm_weight, k_norm_weight,

@@ -109,11 +109,17 @@ def check_codes(codes, y, scale, rel=None):
     """Kernel e4m3 codes against fp64 y / scale. Returns (unexplained, explained_flips): a code
     that differs from the fp64 value's rounding counts as explained only when a rounding boundary
     lies within the bound of that value."""
-    codes = np.asarray(codes).astype(np.uint8)
     rel = rel_bound(y.shape[-1]) if rel is None else rel
     s = float(np.float32(scale))
     v = y / s
     b = ((1 + rel) * (1 + U) ** 2 - 1) * np.abs(v) + TINY / abs(s)
+    return check_codes_within(codes, v, b)
+
+
+def check_codes_within(codes, v, b):
+    """Kernel e4m3 codes against fp64 values v whose kernel-side fp32 value is within b of v.
+    Returns (unexplained, explained_flips) as check_codes does."""
+    codes = np.asarray(codes).astype(np.uint8)
     lo, hi = _ordinal(e4m3_code(v - b)), _ordinal(e4m3_code(v + b))
     k = _ordinal(codes)
     ok = (k >= lo) & (k <= hi)
