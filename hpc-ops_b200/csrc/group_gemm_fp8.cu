@@ -501,8 +501,10 @@ int run(int mode, const void* x, const void* w, const int* seqlens, const int* c
   }
 }
 
-// activation-scale column granule from the average rows per group
-// (reference src/fuse_moe/entry.cc:525-543; replicated in group_gemm_blockwise_fp8.cu:384-456)
+// Activation-scale column granule from the average rows per group (reference
+// src/fuse_moe/entry.cc:525-543). The one rule of the library: the grouped GEMMs, the FusedMoE route
+// and, through hpc_scale_tile_from_avg, reformat_x_scale and the Python host code all take it from
+// here, so a layout written by one is the layout read by the other.
 int scale_tile_from_avg(int avg) {
   if (avg <= 8) return 8;
   if (avg <= 16) return 16;
@@ -519,6 +521,10 @@ int scale_tile_from_avg(int avg) {
 }  // namespace b200
 
 using namespace b200;  // NOLINT
+
+extern "C" int hpc_scale_tile_from_avg(int num_seq_per_group_avg) {
+  return ggemm::scale_tile_from_avg(num_seq_per_group_avg);
+}
 
 // replaces reference src/group_gemm/group_gemm.h:22-29 (group_gemm_blockwise_fp8_async). The
 // tmas / tiles / cu_tiles / task_map / num_waves / update_tma / use_pdl arguments are accepted for

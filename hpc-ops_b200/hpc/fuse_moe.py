@@ -20,11 +20,8 @@ from ._ffi import (check as _check_rc, lib as _lib, ptr as _ptr, require as _req
 
 
 def _aligned_size(avg: int) -> int:
-    # reference src/fuse_moe/entry.cc:525-543
-    for lim, val in ((8, 8), (16, 16), (32, 32), (48, 48), (64, 64), (96, 48), (128, 32), (144, 48)):
-        if avg <= lim:
-            return val
-    return 64
+    # reference src/fuse_moe/entry.cc:525-543; the rule the route kernel and the GEMMs use
+    return int(_lib.hpc_scale_tile_from_avg(int(avg)))
 
 
 def _check_moe_common(x, gate_up_weight, down_weight, topk_ids, topk_scale):

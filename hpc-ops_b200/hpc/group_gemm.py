@@ -11,16 +11,10 @@ from ._ffi import (check as _check_rc, lib as _lib, ptr as _ptr, require as _req
 
 
 def _scale_tile(avg: int) -> int:
-    # reference src/group_gemm/entry.cc:191-202 (reformat) — 8/16/32/48/64 by average rows
-    if avg <= 8:
-        return 8
-    if avg <= 16:
-        return 16
-    if avg <= 32:
-        return 32
-    if avg <= 48:
-        return 48
-    return 64
+    # The granule group_gemm_blockwise_fp8 reads the layout with (csrc/group_gemm_fp8.cu
+    # scale_tile_from_avg). The reference's reformat entry (src/group_gemm/entry.cc:191-202) uses 64
+    # for every avg > 48, which its GEMM does not for 65 <= avg <= 144.
+    return int(_lib.hpc_scale_tile_from_avg(int(avg)))
 
 
 def _check_common(x, weight, seqlens, cu_seqlens):

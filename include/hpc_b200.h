@@ -143,6 +143,10 @@ int hpc_group_gemm_fp8_async(void* y_ptr, const void* x_ptr, const void* w_ptr,
                              void* cu_tiles_ptr, void* task_map_ptr, int num_waves, int num_group,
                              int m, int n, int k, int num_seq_per_group_avg, int update_tma,
                              int use_pdl, cudaStream_t stream);
+/* Column granule of the transposed activation-scale layout for a given average of rows per group:
+ * 8 / 16 / 32 / 48 / 64 up to 64 rows, then 48 (<= 96), 32 (<= 128), 48 (<= 144) and 64. The blockwise
+ * GEMMs read that layout with this granule; pass it as `tilem` to hpc_reformat_x_scale_async. */
+int hpc_scale_tile_from_avg(int num_seq_per_group_avg);
 /* replaces reference src/group_gemm/group_gemm.h:31-33 (row-major [m, n] scales -> transposed,
  * tile-padded [n, m] layout the blockwise GEMM reads) */
 int hpc_reformat_x_scale_async(void* output_ptr, const void* xscale_ptr, const void* seqlens_ptr,

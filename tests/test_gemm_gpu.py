@@ -1,5 +1,6 @@
-"""GPU parity tests of the BF16 x FP32 route GEMM (grid of reference tests/test_gemm_bf16xfp32.py:14-45;
-that test runs on sm_90 upstream)."""
+"""GPU parity tests of the BF16 x FP32 route GEMM at the reference's tolerances (grid of reference
+tests/test_gemm_bf16xfp32.py:14-45). The per-element fp64 checks at every split are in
+tests/test_gemm_exact_gpu.py."""
 import pytest
 import torch
 

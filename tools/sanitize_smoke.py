@@ -114,6 +114,27 @@ def main():
         y = hpc.gemm_bf16xfp32(x, wh, wl, scale, True, True, ws)
         ref = og.gemm_split_exact(x, wh, wl, scale)
         assert float(((y.double() - ref).abs().max() / ref.abs().max())) < 1e-4
+        # split 8 over 4 K steps (k = 200, ragged): CTAs 4..7 of every cluster have no K step
+        from oracle import gemm_exact as ge
+        x, _, wh, wl, scale = og.make_inputs(129, 192, 200, device="cuda")
+        y = torch.empty((129, 192), device="cuda")
+        hpc._ffi.check(hpc._ffi.lib.hpc_gemm_bf16xfp32_async(
+            hpc._ffi.ptr(y), None, None, hpc._ffi.ptr(x), hpc._ffi.ptr(wh), hpc._ffi.ptr(wl), 129, 192, 200,
+            scale, 1, 8, 128, 1, 0, hpc._ffi.stream_of(x)), "gemm_bf16xfp32")
+        ye, _, E = ge.route_exact(x.cpu(), wh.cpu(), wl.cpu(), scale, 8)
+        ge.route_accumulation_ratio(y.cpu(), ye, E)
+        # scatter grouped GEMM with indices the gather clamps into the pool (-1, pool_rows)
+        from synth import gemm_exact as sg
+        d = sg.make_scatter_case(sg.SCATTER_CASES[0])
+        c = cuda(d)
+        G = d["w"].size(0)
+        z = torch.zeros(G + 1, dtype=torch.int32, device="cuda")
+        out = torch.ops.hpc.group_gemm_fp8_scatter_cp_async(c["pool"], c["w"], c["y_scale"], c["row_indices"],
+                                                            c["seqlens"], c["cu_seqlens"], z[:G], z, False)
+        compact = d["pool"][ge.scatter_rows(d["row_indices"], d["pool"].size(0))]
+        rows = ge.rows_to_check(d["seqlens"], d["cu_seqlens"], 1, 1)
+        ye, B, _ = ge.grouped_pertensor_exact(compact, d["w"], d["seqlens"], d["cu_seqlens"], d["y_scale"], rows)
+        ge.check_down(out.cpu()[rows], ye, B)
         print("gemm ok")
     if "rope" in which:
         d = sr.make_inputs(3, True, None, 8, 2, 128, seed=7, max_num_kv_blocks=32)
