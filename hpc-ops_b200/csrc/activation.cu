@@ -10,6 +10,9 @@
 //                       the per-expert padded (DeepEP low-latency) layout [E * T_max, 2C], valid rows
 //                       only, per-tensor or 1x128 blockwise e4m3 (reference activation.cu:203-280 and
 //                       :358-433; there every thread visits every padded row)
+//   blockwise_fp8_quant : bf16 [M, K] -> e4m3 [M, K] and 1x128 scales f32 [M, K / 128], the
+//                       blockwise arithmetic above without the SiLU * mul (no reference counterpart:
+//                       the activation side of the blockwise FP8 GEMMs)
 //   gather_rows       : dst[i, :] = src[row_indices[i], :]   (the A-operand gather of the reference's
 //                       scatter grouped GEMM, src/group_gemm/cp_async/group_gemm_fp8_scatter.cu:20-46,
 //                       done here as a streaming pre-pass in front of the TMA-fed grouped GEMM)
@@ -139,6 +142,20 @@ __global__ void __launch_bounds__(kThreads)
   }
 }
 
+// One 1x128 block held as 8 values by each of the 16 lanes of a half-warp (`half_mask`): sc =
+// amax / 448 over the block, returns the lane's 8 codes e4m3(v * (1 / (sc + 1e-8))).
+__device__ __forceinline__ uint2 blockwise_quant8(const float (&m)[8], unsigned half_mask,
+                                                  float& sc) {
+  float amax = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; i++) amax = fmaxf(amax, fabsf(m[i]));
+#pragma unroll
+  for (int o = 8; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(half_mask, amax, o));
+  sc = amax / 448.0f;
+  const float inv = 1.0f / (sc + 1e-8f);
+  return quant8(m, inv);
+}
+
 // blockwise: per (row, 128 columns) = 16 lanes x 8 columns, sc = amax / 448,
 // out = e4m3(v * (1 / (sc + 1e-8))), out_scale[row, block] = sc (row-major [E * T_max, C / 128]).
 // vpr is a multiple of 16 and so is every item index a half-warp starts at, so the 16 lanes of a
@@ -161,15 +178,41 @@ __global__ void __launch_bounds__(kThreads)
     const long long r = valid_row(prefix, num_expert, t_max, k);
     float m[8];
     silu_mul8(in + r * (2LL * half_col) + c, half_col, 0, m);
-    float amax = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; i++) amax = fmaxf(amax, fabsf(m[i]));
-#pragma unroll
-    for (int o = 8; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(half_mask, amax, o));
-    const float sc = amax / 448.0f;
-    const float inv = 1.0f / (sc + 1e-8f);
-    *reinterpret_cast<uint2*>(out + r * half_col + c) = quant8(m, inv);
+    float sc;
+    *reinterpret_cast<uint2*>(out + r * half_col + c) = blockwise_quant8(m, half_mask, sc);
     if ((lane & 15) == 0) out_scale[r * (half_col >> 7) + (c >> 7)] = sc;
+  }
+}
+
+// bf16 [M, K] (row stride `ld` elements) -> e4m3 [M, K] and sc f32 [M, K / 128], the arithmetic of
+// masked_act_mul_and_blockwise_quant_kernel without the SiLU * mul. vpr = K / 8 is a multiple of 16,
+// so the 16 lanes of a 128-column block are again the 16 lanes of one half-warp.
+__global__ void __launch_bounds__(kThreads)
+    blockwise_fp8_quant_kernel(uint8_t* __restrict__ out, float* __restrict__ out_scale,
+                               const __nv_bfloat16* __restrict__ in, long long num_row, int num_col,
+                               long long ld) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int vpr = num_col >> 3;
+  const long long total = num_row * vpr;
+  const int lane = threadIdx.x & 31;
+  const unsigned half_mask = 0xffffu << (lane & 16);
+  for (long long v = static_cast<long long>(blockIdx.x) * kThreads + threadIdx.x; v < total;
+       v += static_cast<long long>(gridDim.x) * kThreads) {
+    const long long r = v / vpr;
+    const int c = static_cast<int>(v - r * vpr) << 3;
+    const uint4 raw = ld_nc_v4(in + r * ld + c);
+    const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&raw);
+    float m[8];
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+      const float2 f = __bfloat1622float2(h2[i]);
+      m[2 * i] = f.x;
+      m[2 * i + 1] = f.y;
+    }
+    float sc;
+    *reinterpret_cast<uint2*>(out + r * num_col + c) = blockwise_quant8(m, half_mask, sc);
+    if ((lane & 15) == 0) out_scale[r * (num_col >> 7) + (c >> 7)] = sc;
   }
 }
 
@@ -340,6 +383,33 @@ extern "C" int hpc_masked_act_mul_and_blockwise_quant_async(
       static_cast<const __nv_bfloat16*>(input_ptr), num_per_expert_ptr,
       num_total_tokens / num_tokens_per_expert, num_tokens_per_expert, num_intermediate_size);
   HPC_CUDA_CHECK(cudaGetLastError());
+  return HPC_OK;
+}
+
+// No reference counterpart: the 1x128 activation quantiser in front of the blockwise FP8 GEMMs.
+// input bf16 [num_row, num_col] with row stride input_ld elements; output e4m3 [num_row, num_col]
+// and output_scale f32 [num_row, num_col / 128], both contiguous.
+extern "C" int hpc_blockwise_fp8_quant_async(void* output_ptr, float* output_scale_ptr,
+                                             const void* input_ptr, int num_row, int num_col,
+                                             int64_t input_ld, cudaStream_t stream) {
+  HPC_REQUIRE(num_row >= 0 && num_col > 0 && num_col % 128 == 0,
+              "blockwise_fp8_quant: shape [%d, %d] needs rows >= 0 and columns a positive multiple "
+              "of 128", num_row, num_col);
+  HPC_REQUIRE(input_ld >= num_col && input_ld % 8 == 0,
+              "blockwise_fp8_quant: row stride %lld must be >= %d and a multiple of 8 elements",
+              static_cast<long long>(input_ld), num_col);
+  HPC_REQUIRE((reinterpret_cast<uintptr_t>(input_ptr) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(output_ptr) & 7) == 0 &&
+                  (reinterpret_cast<uintptr_t>(output_scale_ptr) & 3) == 0,
+              "blockwise_fp8_quant: input must be 16-byte, output 8-byte and output_scale 4-byte "
+              "aligned");
+  if (num_row == 0) return HPC_OK;
+  const long long items = static_cast<long long>(num_row) * (num_col / 8);
+  HPC_CUDA_CHECK(launch_pdl(act::blockwise_fp8_quant_kernel, dim3(act::stream_grid(items)),
+                            dim3(act::kThreads), 0, stream, 1, static_cast<uint8_t*>(output_ptr),
+                            output_scale_ptr, static_cast<const __nv_bfloat16*>(input_ptr),
+                            static_cast<long long>(num_row), num_col,
+                            static_cast<long long>(input_ld)));
   return HPC_OK;
 }
 

@@ -65,15 +65,6 @@ constexpr int kSmemBytes = kStages * kStageBytes + (kMaxGroups + 4 + 3 * kMaxGro
                            (2 * kStages + 2 * kTileQ) * 8 + kTileQ * 4;
 static_assert(kSmemBytes <= 227 * 1024, "bf16 grouped GEMM smem exceeds the sm_90 per-block limit");
 
-template <uint32_t kRegs>
-__device__ __forceinline__ void setmaxnreg_inc() {
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs));
-}
-template <uint32_t kRegs>
-__device__ __forceinline__ void setmaxnreg_dec() {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs));
-}
-
 template <bool kFused>
 __global__ void __launch_bounds__(kThreads, 1)
     group_gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a,

@@ -112,6 +112,26 @@ def _masked_act_mul_and_blockwise_quant_impl(input, num_per_expert, output, outp
     return output, output_scale
 
 
+def _blockwise_fp8_quant_impl(input, output, output_scale):
+    what = "blockwise_fp8_quant"
+    _require(input.is_cuda and input.dtype == torch.bfloat16 and input.dim() == 2,
+             f"{what}: input must be a bfloat16 [M, K] cuda tensor")
+    m, k = input.shape
+    _require(k % 128 == 0 and k > 0, f"{what}: K ({k}) must be a positive multiple of 128")
+    _require(input.stride(1) == 1 and (m <= 1 or input.stride(0) % 8 == 0),
+             f"{what}: input rows must be contiguous with a row stride that is a multiple of 8")
+    if output is None:
+        output = torch.empty((m, k), dtype=torch.float8_e4m3fn, device=input.device)
+    if output_scale is None:
+        output_scale = torch.empty((m, k // 128), dtype=torch.float32, device=input.device)
+    _check_out(what, "output", output, (m, k), torch.float8_e4m3fn, input.device)
+    _check_out(what, "output_scale", output_scale, (m, k // 128), torch.float32, input.device)
+    ld = input.stride(0) if m > 1 else k
+    _check_rc(_lib.hpc_blockwise_fp8_quant_async(_ptr(output), _ptr(output_scale), _ptr(input), m,
+                                                  k, ld, _stream_of(input)), what)
+    return output, output_scale
+
+
 _ops.define("act_mul_and_quant(Tensor input, Tensor scale, bool use_bf16_mul, Tensor? output) -> "
             "(Tensor)")
 _ops.impl("act_mul_and_quant", _act_mul_and_quant_impl, "CUDA")
@@ -123,6 +143,9 @@ _ops.impl("masked_act_mul_and_quant", _masked_act_mul_and_quant_impl, "CUDA")
 _ops.define("masked_act_mul_and_blockwise_quant(Tensor input, Tensor num_per_expert, Tensor? output, "
             "Tensor? output_scale) -> (Tensor output, Tensor output_scale)")
 _ops.impl("masked_act_mul_and_blockwise_quant", _masked_act_mul_and_blockwise_quant_impl, "CUDA")
+_ops.define("blockwise_fp8_quant(Tensor input, Tensor? output, Tensor? output_scale) -> "
+            "(Tensor output, Tensor output_scale)")
+_ops.impl("blockwise_fp8_quant", _blockwise_fp8_quant_impl, "CUDA")
 
 
 def act_mul_and_quant(gate_up: Tensor, scale: Tensor, use_bf16_mul: bool = True,
@@ -162,6 +185,19 @@ def masked_act_mul_and_blockwise_quant(gate_up: Tensor, num_per_expert: Tensor,
                                                             output_scale)
 
 
+def blockwise_fp8_quant(input: Tensor, output: Optional[Tensor] = None,
+                        output_scale: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
+    """1x128 blockwise FP8 quantisation of bf16 activations `input` [M, K] (K % 128 == 0, rows
+    contiguous, row stride a multiple of 8 elements). Per (row, 128 columns), in fp32:
+    sc = amax|v| / 448, out = e4m3_rn_satfinite(v * (1 / (sc + 1e-8))) -- the arithmetic of
+    masked_act_mul_and_blockwise_quant without the SiLU * mul. Returns (out e4m3 [M, K],
+    sc f32 [M, K / 128]), both contiguous: the (x, x_scale) pair gemm_blockwise_fp8 and
+    fuse_moe_blockwise_fp8 take. Caller-given outputs must have exactly these dtypes, shapes and the
+    input's device, and be contiguous. No allocation beyond the outputs and no host
+    synchronisation: capturable."""
+    return torch.ops.hpc.blockwise_fp8_quant(input, output, output_scale)
+
+
 @torch.library.register_fake("hpc::act_mul_and_quant")
 def _act_mul_and_quant_fake(input, scale, use_bf16_mul, output):
     shape = list(input.shape)
@@ -185,3 +221,10 @@ def _masked_act_mul_and_blockwise_quant_fake(input, num_per_expert, output, outp
     n, c = input.shape[0], input.shape[1] // 2
     return (torch.empty(n, c, dtype=torch.float8_e4m3fn, device=input.device),
             torch.empty(n, c // 128, dtype=torch.float32, device=input.device))
+
+
+@torch.library.register_fake("hpc::blockwise_fp8_quant")
+def _blockwise_fp8_quant_fake(input, output, output_scale):
+    m, k = input.shape
+    return (torch.empty(m, k, dtype=torch.float8_e4m3fn, device=input.device),
+            torch.empty(m, k // 128, dtype=torch.float32, device=input.device))

@@ -1,4 +1,7 @@
-"""BF16 x FP32 route GEMM (API of reference hpc/gemm.py)."""
+"""BF16 x FP32 route GEMM (API of reference hpc/gemm.py) and the dense blockwise FP8 GEMM of the
+linear layers of a blockwise-FP8 checkpoint (no reference counterpart)."""
+from typing import Optional
+
 import torch
 from torch import Tensor
 
@@ -65,3 +68,58 @@ def _gemm_bf16xfp32_fake(a, b_high, b_low, scale, use_fp32_output=False, use_spl
                          split_flag=None):
     dt = torch.float32 if use_fp32_output else a.dtype
     return torch.empty((a.shape[0], b_high.shape[0]), dtype=dt, device=a.device)
+
+
+def _gemm_blockwise_fp8_impl(x, x_scale, weight, weight_scale, output):
+    what = "gemm_blockwise_fp8"
+    _require(x.dim() == 2 and weight.dim() == 2, f"{what}: x and weight must be 2-D")
+    m, k = x.shape
+    n = weight.size(0)
+    _require(k % 128 == 0 and 128 <= k <= 65536,
+             f"{what}: K ({k}) must be a multiple of 128 in [128, 65536]")
+    _require(n > 0 and n % 8 == 0, f"{what}: N ({n}) must be a positive multiple of 8")
+    dev = x.device
+    _require(x.is_cuda, f"{what}: x must be a cuda tensor")
+    for name, t, shape, dtype in (("x", x, (m, k), torch.float8_e4m3fn),
+                                  ("x_scale", x_scale, (m, k // 128), torch.float32),
+                                  ("weight", weight, (n, k), torch.float8_e4m3fn),
+                                  ("weight_scale", weight_scale, ((n + 127) // 128, k // 128),
+                                   torch.float32)):
+        _require(t.dtype == dtype and tuple(t.shape) == shape and t.device == dev and t.is_contiguous(),
+                 f"{what}: {name} must be a contiguous {dtype} tensor of shape {list(shape)} on "
+                 f"{dev}, got {t.dtype} {list(t.shape)} on {t.device}")
+    if output is None:
+        output = torch.empty((m, n), dtype=torch.bfloat16, device=dev)
+    _require(output.dtype == torch.bfloat16 and tuple(output.shape) == (m, n) and output.device == dev
+             and output.is_contiguous(),
+             f"{what}: output must be a contiguous bfloat16 tensor of shape {[m, n]} on {dev}")
+    _check_rc(_lib.hpc_gemm_blockwise_fp8_async(_ptr(output), _ptr(x), _ptr(x_scale), _ptr(weight),
+                                                _ptr(weight_scale), m, n, k, _stream_of(x)), what)
+    return output
+
+
+_ops.define("gemm_blockwise_fp8(Tensor x, Tensor x_scale, Tensor weight, Tensor weight_scale, "
+            "Tensor? output) -> (Tensor)")
+_ops.impl("gemm_blockwise_fp8", _gemm_blockwise_fp8_impl, "CUDA")
+
+
+def gemm_blockwise_fp8(x: Tensor, x_scale: Tensor, weight: Tensor, weight_scale: Tensor,
+                       output: Optional[Tensor] = None) -> Tensor:
+    """Dense block-scaled FP8 linear layer: y = x . weight^T in bf16 [M, N].
+      x e4m3 [M, K] and x_scale f32 [M, K / 128] (as blockwise_fp8_quant returns them);
+      weight e4m3 [N, K] (nn.Linear layout) and weight_scale f32 [ceil(N / 128), K / 128] (the
+      checkpoint's weight_scale_inv as stored, no padding); all contiguous, 16-byte aligned.
+    K % 128 == 0 with 128 <= K <= 65536, N % 8 == 0, any M >= 0.
+    Arithmetic, per 128-column K block kb in ascending order: P = the e4m3 tensor-core products
+    accumulated over the block's four k = 32 steps from zero; acc = fmaf(P, fl32(x_scale[m, kb] *
+    weight_scale[n // 128, kb]), acc). When the problem is split over K (small M; see
+    hpc._ffi.lib.hpc_gemm_blockwise_fp8_config) each split does this over its contiguous share of
+    the K blocks and the partials are added in fp32 in split order. y = bf16_rn(acc).
+    Deterministic: two calls give identical bits. A caller-given `output` is overwritten entirely.
+    No allocation beyond the output and no host synchronisation: capturable."""
+    return torch.ops.hpc.gemm_blockwise_fp8(x, x_scale, weight, weight_scale, output)
+
+
+@torch.library.register_fake("hpc::gemm_blockwise_fp8")
+def _gemm_blockwise_fp8_fake(x, x_scale, weight, weight_scale, output=None):
+    return torch.empty((x.shape[0], weight.shape[0]), dtype=torch.bfloat16, device=x.device)

@@ -195,6 +195,32 @@ int hpc_masked_act_mul_and_blockwise_quant_async(void* output_ptr, float* output
                                                  const int* num_per_expert_ptr,
                                                  int num_total_tokens, int num_intermediate_size,
                                                  int num_tokens_per_expert, cudaStream_t stream);
+/* 1x128 blockwise activation quantiser, no reference counterpart: input bf16 [num_row, num_col]
+ * (elements of a row contiguous, input_ld elements between rows, a multiple of 8, 16-byte aligned
+ * base), num_col % 128 == 0. Per (row, 128 columns), in fp32: sc = amax / 448, output e4m3
+ * [num_row, num_col] = e4m3_rn_satfinite(v * (1 / (sc + 1e-8))), output_scale f32 row-major
+ * [num_row, num_col / 128] = sc: the x / x_scale pair of hpc_gemm_blockwise_fp8_async and of the
+ * blockwise FusedMoE. num_row = 0 launches nothing. PDL launch, no allocation or host
+ * synchronisation: capturable. */
+int hpc_blockwise_fp8_quant_async(void* output_ptr, float* output_scale_ptr, const void* input_ptr,
+                                  int num_row, int num_col, int64_t input_ld, cudaStream_t stream);
+
+/* ---- dense blockwise FP8 GEMM ---------------------------------------------------------------------
+ * No reference counterpart: the linear layers of a blockwise-FP8 checkpoint.
+ *   y [m, n] bf16 = x [m, k] e4m3 . w [n, k]^T e4m3 with x_scale f32 [m, k / 128] and w_scale f32
+ *   [ceil(n / 128), k / 128], all contiguous and 16-byte aligned.
+ * Per 128-column K block kb in ascending order: P = e4m3 wgmma products accumulated over the block's
+ * four k = 32 steps from zero, acc = fmaf(P, fl32(x_scale[m, kb] * w_scale[n / 128, kb]), acc); with
+ * a K split each split does this over its contiguous share of the K blocks and the split partials
+ * are added in fp32 in split order; y = bf16_rn(acc). Deterministic. k % 128 == 0, 128 <= k <=
+ * 65536, n % 8 == 0 (a ragged last weight-scale block is allowed), any m >= 0 (0 launches nothing),
+ * checked before any launch. PDL launch, no allocation or host synchronisation: capturable.
+ * hpc_gemm_blockwise_fp8_config returns the K split (1, 2, 4 or 8; the tile is always 128 x 128)
+ * the launcher picks for a shape on the current device. */
+int hpc_gemm_blockwise_fp8_config(int m, int n, int k);
+int hpc_gemm_blockwise_fp8_async(void* y_ptr, const void* x_ptr, const float* x_scale_ptr,
+                                 const void* w_ptr, const float* w_scale_ptr, int m, int n, int k,
+                                 cudaStream_t stream);
 
 /* ---- fused RMSNorm -> FP8 --------------------------------------------------------------------------
  * replaces reference src/normalization/fused_rmsnorm_with_scale.h. input bf16 [batch_size,

@@ -123,6 +123,17 @@ def main():
             scale, 1, 8, 128, 1, 0, hpc._ffi.stream_of(x)), "gemm_bf16xfp32")
         ye, _, E = ge.route_exact(x.cpu(), wh.cpu(), wl.cpu(), scale, 8)
         ge.route_accumulation_ratio(y.cpu(), ye, E)
+        # 1x128 quantiser -> dense blockwise FP8 GEMM, split 8 over 17 K blocks, ragged N = 576
+        from oracle import gemm_blockwise as obw
+        from synth import gemm_blockwise as sbw
+        a = sbw.quant_input(3, 2176, seed=1).cuda()
+        q, qs = hpc.blockwise_fp8_quant(a)
+        assert obw.quant_mismatch(q.cpu(), qs.cpu(), *obw.quant(a.cpu())) == (0, 0)
+        d = sbw.make_inputs(sbw.CASES[4])
+        c = cuda(d)
+        y = hpc.gemm_blockwise_fp8(c["x"], c["xs"], c["w"], c["ws"])
+        split = hpc._ffi.lib.hpc_gemm_blockwise_fp8_config(3, 576, 2176)
+        obw.check(y.cpu(), *obw.gemm_exact(d["x"], d["xs"], d["w"], d["ws"], split)[:2])
         # scatter grouped GEMM with indices the gather clamps into the pool (-1, pool_rows)
         from synth import gemm_exact as sg
         d = sg.make_scatter_case(sg.SCATTER_CASES[0])
