@@ -1,5 +1,6 @@
 """One small invocation of every hot-path op (decode both quant types, prefill both, bf16 prefill
-dense and paged, blockwise + per-tensor MoE, bf16 MoE, route GEMM, W=1 allreduce, rope, the Stem mask stages,
+dense and paged, blockwise + per-tensor MoE, bf16 MoE, route GEMM, allreduce with a simulated
+peer (P2P high-throughput, Lamport one-shot and two-shot), rope, the Stem mask stages,
 fused RMSNorm -> FP8, the masked activation quantisers and the speculative sampler),
 meant to run under compute-sanitizer:
 
@@ -147,6 +148,29 @@ def main():
         ye, B, _ = ge.grouped_pertensor_exact(compact, d["w"], d["seqlens"], d["cu_seqlens"], d["y_scale"], rows)
         ge.check_down(out.cpu()[rows], ye, B)
         print("gemm ok")
+    if "allreduce" in which:
+        from oracle import allreduce_exact as ox
+        from synth import allreduce as sa
+        # the P2P transports with a simulated peer on one device: high-throughput (mode 2), then
+        # the Lamport kernel one-shot and two-shot, so memcheck sees every peer address
+        c = sa.make_case("signature", 2, 6, 264, seed=1)
+        args = (c["xs"], c["residual"], c["weight"], c["eps"])
+        sim = sa.HtSim(c["xs"], 264)
+        res, w = c["residual"].cuda(), c["weight"].cuda()
+        ores = torch.empty_like(res)
+        for rank in range(2):
+            sim.launch(rank, 3 * rank, 3 * rank + 3, res[3 * rank:], w, c["eps"], ores[3 * rank:], 1)
+        torch.cuda.synchronize()
+        assert ox.check(ores.cpu(), sim.outs[1].cpu(), *args)["ok"]
+        for proto in (0, 1):
+            c = sa.make_case("lamport", 2, 5, 264, seed=2)
+            args = (c["xs"], c["residual"], c["weight"], c["eps"])
+            out = torch.empty(5, 264, dtype=torch.bfloat16, device="cuda")
+            ores = torch.empty_like(out)
+            sa.ll_sim(*args, 1, proto, sa.ll_buf_bytes(5, 2, 264, True), out, ores)
+            torch.cuda.synchronize()
+            assert ox.check(ores.cpu(), out.cpu(), *args, kernel="ll")["ok"]
+        print("allreduce ok")
     if "rope" in which:
         d = sr.make_inputs(3, True, None, 8, 2, 128, seed=7, max_num_kv_blocks=32)
         c = cuda(d)
