@@ -4,6 +4,7 @@ Implemented in this build (sm_90a):
   * attention_decode_fp8            — quant_type QPERTOKEN_PERHEAD_KPERTENSOR_VPERTENSOR and
                                       QPERTOKEN_PERHEAD_KPERTOKEN_PERHEAD_VPERHEAD (in-cache k scales)
   * attention_decode_bf16           — pages of 16 / 32 / 64 tokens, mtp 0..4
+  * attention_decode_mla_bf16       — absorbed MLA (576 / 512 latent head) over a paged bf16 cache
   * attention_with_kvcache_blocksparse_prefill_fp8 / attention_with_kvcache_prefill_fp8 (dense)
   * attention_prefill_bf16 (varlen causal self-attention on contiguous q/k/v) and
     attention_with_kvcache_prefill_bf16 (causal, chunked, prefill over the paged bf16 cache,
@@ -233,6 +234,79 @@ def _attention_decode_bf16_impl(
     return y
 
 
+_MLA_DQK = 576
+_MLA_DV = 512
+_MLA_HEADS = (8, 16, 32, 64, 128)
+
+
+def mla_num_query_tiles(num_head_q: int, mtp: int) -> int:
+    """T = ceil(H * (mtp + 1) / 64): the 64-row query tiles of one request, the `num_head_kv` an
+    MLA decode task map is built with."""
+    return (num_head_q * (mtp + 1) + 63) // 64
+
+
+def _mla_workspace_floats(num_total_ctas: int) -> int:
+    # split-chunk partials [2C, 64, 512] and LSEs [2C, 64], the rotated walk's carry [C, 256*128+512]
+    return 2 * num_total_ctas * 64 * (_MLA_DV + 1) + num_total_ctas * (256 * 128 + 512)
+
+
+def _attention_decode_mla_bf16_impl(q, kv_cache, block_ids, num_seq_kvcache, softmax_scale, mtp,
+                                    new_kv_included, task_map=None, output=None):
+    who = "attention_decode_mla_bf16"
+    _require(q.is_cuda and kv_cache.is_cuda and block_ids.is_cuda and num_seq_kvcache.is_cuda,
+             f"{who}: q, kv_cache, block_ids and num_seq_kvcache must be cuda tensors")
+    _require(q.dtype == torch.bfloat16 and kv_cache.dtype == torch.bfloat16,
+             f"{who}: q and kv_cache must be bfloat16")
+    _require(block_ids.dtype == torch.int32 and block_ids.dim() == 2 and block_ids.is_contiguous(),
+             f"{who}: block_ids must be contiguous int32 [num_batch, max_blocks]")
+    _require(num_seq_kvcache.dtype == torch.int32 and num_seq_kvcache.dim() == 1
+             and num_seq_kvcache.is_contiguous(), f"{who}: num_seq_kvcache must be contiguous int32 [B]")
+    _require(mtp in (0, 1, 2, 3), f"{who}: mtp must be 0, 1, 2 or 3")
+    num_batch = num_seq_kvcache.size(0)
+    _require(1 <= num_batch <= 2048, f"{who}: batch must be 1..2048")
+    _require(block_ids.size(0) == num_batch, f"{who}: block_ids must have num_batch rows")
+    num_seq_q = mtp + 1
+    _require(q.dim() == 3 and q.size(0) == num_batch * num_seq_q,
+             f"{who}: q must be [num_batch * (mtp + 1), H, 576]")
+    num_head_q = q.size(1)
+    _require(num_head_q in _MLA_HEADS, f"{who}: num heads must be one of {_MLA_HEADS}")
+    _require(q.size(2) == _MLA_DQK, f"{who}: q head dim must be 576")
+    _require(q.stride(2) == 1 and q.stride(1) == _MLA_DQK,
+             f"{who}: q must be contiguous in (head, dim)")
+    _require(kv_cache.dim() == 3 and kv_cache.size(2) == _MLA_DQK and kv_cache.stride(2) == 1,
+             f"{who}: kv_cache must be [num_blocks, 64, 576] with contiguous rows")
+    _require(kv_cache.size(1) == 64, f"{who}: page size must be 64")
+    y = output
+    rows = num_batch * num_seq_q
+    if y is None:
+        y = torch.empty((rows, num_head_q, _MLA_DV), dtype=torch.bfloat16, device=q.device)
+    else:
+        _require(y.is_cuda and y.device == q.device and y.dtype == torch.bfloat16,
+                 f"{who}: output must be bfloat16 on q's device")
+        _require(tuple(y.shape) == (rows, num_head_q, _MLA_DV),
+                 f"{who}: output must have shape [num_batch * (mtp + 1), H, 512]")
+        _require(y.stride(2) == 1 and y.stride(1) == _MLA_DV
+                 and (rows == 1 or y.stride(0) >= num_head_q * _MLA_DV),
+                 f"{who}: output rows must be [H, 512] contiguous and must not overlap")
+        _require(y.data_ptr() % 16 == 0 and (rows == 1 or y.stride(0) % 8 == 0),
+                 f"{who}: output and its row stride must be 16-byte aligned")
+    num_tiles = mla_num_query_tiles(num_head_q, mtp)
+    if task_map is None:
+        task_map = get_attention_decode_task_workspace(
+            num_batch, int(block_ids.size(1)) * 64 + num_seq_q, num_tiles, min_process_len=512,
+            device=q.device)
+        _assign_task_cuda(num_seq_kvcache, num_tiles, num_seq_q, new_kv_included, 512, task_map)
+    num_total_ctas = _num_total_ctas(q.device)
+    ws = torch.empty(_mla_workspace_floats(num_total_ctas), dtype=torch.float32, device=q.device)
+    chunk_base = torch.empty(num_batch * num_tiles, dtype=torch.int32, device=q.device)
+    _check_rc(_lib.hpc_attention_decode_mla_bf16_async(
+        _ptr(y), _ptr(ws), _ptr(chunk_base), _ptr(task_map), _ptr(q), _ptr(kv_cache),
+        _ptr(block_ids), num_batch, num_seq_q, num_head_q, q.size(2), kv_cache.size(0),
+        kv_cache.size(1), block_ids.size(1), y.stride(0), q.stride(0), kv_cache.stride(0),
+        kv_cache.stride(1), float(softmax_scale), num_total_ctas, _stream_of(q)), who)
+    return y
+
+
 def _assign_task_cpu(num_seq_kvcache, num_head_kv, num_seq_q, new_kv_included, min_process_len,
                      placeholder=None, num_total_ctas: _Optional[int] = None):
     """CPU scheduler -> packed host task map int8 [rows, 48] (reference entry.cc:727-778)."""
@@ -456,6 +530,12 @@ _ops.define(
 _ops.impl("attention_decode_bf16", _attention_decode_bf16_impl, "CUDA")
 
 _ops.define(
+    "attention_decode_mla_bf16(Tensor q, Tensor kv_cache, Tensor block_ids, Tensor num_seq_kvcache, "
+    "float softmax_scale, int mtp, bool new_kv_included, Tensor? task_map, Tensor? output) -> "
+    "(Tensor)")
+_ops.impl("attention_decode_mla_bf16", _attention_decode_mla_bf16_impl, "CUDA")
+
+_ops.define(
     "attention_decode_fp8(Tensor q, Tensor! kcache, Tensor! vcache, Tensor block_ids, Tensor "
     "num_seq_kvcache, Tensor qscale, Tensor kscale, Tensor vscale, int mtp, bool "
     "new_kv_included, int quant_type, bool "
@@ -604,6 +684,41 @@ def attention_decode_bf16(
         q, kcache, vcache, block_ids, num_seq_kvcache, mtp, new_kv_included, splitk, task_map,
         split_flag, output,
     )
+
+
+def attention_decode_mla_bf16(
+    q: Tensor,
+    kv_cache: Tensor,
+    block_ids: Tensor,
+    num_seq_kvcache: Tensor,
+    softmax_scale: float,
+    mtp: int = 0,
+    new_kv_included: bool = False,
+    task_map: Tensor = None,
+    output: Tensor = None,
+) -> Tensor:
+    """Absorbed multi-head latent attention (MLA) decode over a paged bf16 latent cache.
+
+      q           [B * (mtp + 1), H, 576] bfloat16, contiguous in (head, dim); each head is
+                  [q_nope . W_UK (512) | q_pe after RoPE (64)]. H in {8, 16, 32, 64, 128}.
+      kv_cache    [num_blocks, 64, 576] bfloat16; each row is [kv_c (512) | k_pe after RoPE (64)].
+                  Rows must be contiguous; the token and block strides may be any multiple of 8
+                  elements (a view into a wider allocation works). Slots past a request's last
+                  token never reach the output, whatever they hold (NaN included).
+      block_ids   [B, max_blocks] int32;  num_seq_kvcache [B] int32, B <= 2048
+      softmax_scale  used as given: s = (q . k) * softmax_scale (DeepSeek-V3: mscale^2 / sqrt(192))
+      mtp         0..3; MTP row sq of a request with n keys sees keys <= n - (mtp + 1) + sq, where n
+                  is num_seq_kvcache[b] (+ mtp + 1 unless new_kv_included), as attention_decode_bf16
+      task_map    from get_attention_decode_task_workspace + assign_attention_decode_task built with
+                  num_head_kv = T = mla_num_query_tiles(H, mtp) = ceil(H (mtp + 1) / 64), the
+                  64-row query tiles of a request (None: scheduled on the device inside the call)
+      output      optional bf16 [B * (mtp + 1), H, 512]; rows may be strided (16-byte aligned)
+    Returns y = softmax(s) . kv_cache[..., :512], bf16 [B * (mtp + 1), H, 512]. The launch
+    allocates nothing outside torch's allocator and never synchronises, so it can be captured in a
+    CUDA graph (with a pre-assigned task map)."""
+    return torch.ops.hpc.attention_decode_mla_bf16(
+        q, kv_cache, block_ids, num_seq_kvcache, float(softmax_scale), mtp, new_kv_included,
+        task_map, output)
 
 
 def attention_decode_fp8(
@@ -782,6 +897,14 @@ def _attention_decode_bf16_fake(
     if output is not None:
         return output
     return torch.empty_like(q)
+
+
+@torch.library.register_fake("hpc::attention_decode_mla_bf16")
+def _attention_decode_mla_bf16_fake(q, kv_cache, block_ids, num_seq_kvcache, softmax_scale, mtp,
+                                    new_kv_included, task_map=None, output=None):
+    if output is not None:
+        return output
+    return q.new_empty((q.size(0), q.size(1), _MLA_DV))
 
 
 @torch.library.register_fake("hpc::attention_decode_fp8")

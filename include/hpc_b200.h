@@ -96,6 +96,26 @@ int hpc_attention_decode_bf16_async(
     int64_t vcache_block_stride, int64_t vcache_token_stride, int64_t vcache_head_stride,
     cudaStream_t stream);
 
+/* ---- decode attention: absorbed MLA over a paged bf16 latent cache -----------------------------
+ * y[b * Sq + sq, h, :512] = softmax_k(q[b * Sq + sq, h, :] . kv[k, :] * softmax_scale) . kv[k, :512]
+ * over the n = num_seq_kvcache[b] (+ Sq unless new kv is included) cached tokens of request b; MTP
+ * row sq sees keys k <= n - Sq + sq. q: [B * Sq, H, 576] bf16, heads contiguous (576 apart), row
+ * stride ldQ; kv: [num_kvcache_blocks, 64, 576] bf16 with token / block strides in elements
+ * (multiples of 8); y: [B * Sq, H, 512] bf16 with row stride ldY. H in {8, 16, 32, 64, 128}, Sq
+ * 1..4, B <= 2048. Cache slots past a request's last token never reach y, whatever they hold.
+ *   task_map   : the decode task map built with num_head_kv = T = ceil(H * Sq / 64) (query tiles)
+ *                for the same num_total_ctas (the grid)
+ *   workspace  : fp32, 2 * C * 64 * 513 + C * (256 * 128 + 512) floats for C = num_total_ctas
+ *                (split-chunk partials and LSEs, and the rotated walk's carried state); any contents
+ *   chunk_base : int32 [B * T], any contents
+ * No allocation and no host synchronisation: capturable in a CUDA graph. */
+int hpc_attention_decode_mla_bf16_async(
+    void* y_ptr, void* workspace_ptr, int* chunk_base_ptr, const int* task_map_ptr,
+    const void* q_ptr, const void* kv_ptr, const int* block_ids_ptr, int num_batch,
+    int num_seq_q, int num_head_q, int num_dim_qk, int num_kvcache_blocks, int block_size,
+    int num_seq_max_blocks, int ldY, int ldQ, int64_t kv_block_stride, int64_t kv_token_stride,
+    float softmax_scale, int num_total_ctas, cudaStream_t stream);
+
 /* The two stages of hpc_attention_decode_fp8_async on their own, same argument list: the split-k
  * attention kernel (writes lse / split_out) and the LSE combine (reads them, writes y). The
  * reference launches them back to back inside one launcher

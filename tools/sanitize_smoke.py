@@ -29,7 +29,7 @@ def cuda(d):
 
 def main():
     which = set(sys.argv[1:]) or {"decode", "prefill", "prefill_bf16", "moe", "moe_bf16", "gemm",
-                                  "allreduce", "rope", "stem", "norm_act", "spec"}
+                                  "allreduce", "rope", "stem", "norm_act", "spec", "mla"}
     if "decode" in which:
         B, hkv, hq = 3, 2, 8
         lens = [300, 129, 64]
@@ -250,6 +250,21 @@ def main():
             o = out.cpu().numpy()
             assert ((o >= 0) & (o < 4096) | (o == -1)).all()
         print("spec ok")
+    if "mla" in which:
+        # absorbed MLA decode: two query tiles, a split pair and NaN in the unused cache slots
+        from oracle import attention_mla as oml
+        from synth import attention_mla as sml
+        d = sml.make_case([700, 65], 128, 0, seed=1, num_total_ctas=hpc._ffi.sm_count(),
+                          min_process_len=64)
+        T = oml.num_tiles(128, 1)
+        tm = hpc.get_attention_decode_task_workspace(2, d["block_ids"].size(1) * 64 + 1, T, 64)
+        lens = d["lens_total"].cuda()
+        hpc.assign_attention_decode_task(lens, tm, T, 1, True, 64)
+        y = hpc.attention_decode_mla_bf16(d["q"].cuda(), d["kv"].cuda(), d["block_ids"].cuda(), lens,
+                                          d["scale"], mtp=0, new_kv_included=True, task_map=tm)
+        r = oml.check(y.float().cpu(), d)
+        assert r["ok_a"] and r["ok_b"], r
+        print("mla ok")
     torch.cuda.synchronize()
     print("smoke ok")
 
