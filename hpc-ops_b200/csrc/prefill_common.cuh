@@ -44,6 +44,8 @@ struct Work {
   int num_tile_kv;  // causal extent of this Q tile in KV tiles
 };
 
+// kKvOffsets: p.seqlens_kv holds B + 1 key offsets (cu_seqlens_kv), not B lengths.
+template <bool kKvOffsets = false>
 __device__ __forceinline__ bool decode_work(const Params& p, int w, Work& k) {
   const int per_level = p.num_batch * p.num_head_q;
   if (w >= p.max_q_tiles * per_level) return false;
@@ -54,7 +56,7 @@ __device__ __forceinline__ bool decode_work(const Params& p, int w, Work& k) {
   k.hq = rem - k.b * p.num_head_q;
   const int s0 = p.cu_seqlens_q[k.b];
   k.seq_q = p.cu_seqlens_q[k.b + 1] - s0;
-  k.seq_kv = p.seqlens_kv[k.b];
+  k.seq_kv = kKvOffsets ? p.seqlens_kv[k.b + 1] - p.seqlens_kv[k.b] : p.seqlens_kv[k.b];
   k.q0 = s0 + k.mq * kTile;
   const int left = k.seq_q - k.mq * kTile;
   k.rows = left < kTile ? left : kTile;

@@ -9,6 +9,8 @@ Implemented in this build (sm_90a):
   * attention_prefill_bf16 (varlen causal self-attention on contiguous q/k/v) and
     attention_with_kvcache_prefill_bf16 (causal, chunked, prefill over the paged bf16 cache,
     pages of 16 / 32 / 64 tokens)
+  * attention_prefill_mla_bf16      — un-absorbed MLA prefill (192-wide q / k with a head-shared
+                                      k_pe, 128-wide v), varlen, bottom-right causal
   * get_attention_decode_task_workspace / assign_attention_decode_task (CPU and CUDA)
   * print_attention_decode_task
 The host side does what the reference's torch entry does (validation, scratch allocation, stride
@@ -509,6 +511,63 @@ def _attention_with_kvcache_prefill_bf16_impl(q, kcache, vcache, cu_seqlens_q, b
     return y
 
 
+_MLA_PREFILL_DQK = 192
+_MLA_PREFILL_DV = 128
+_MLA_PREFILL_DPE = 64
+
+
+def _attention_prefill_mla_bf16_impl(q, k_nope, k_pe, v, cu_seqlens_q, cu_seqlens_kv,
+                                     max_seqlen_q, softmax_scale, output=None):
+    who = "attention_prefill_mla_bf16"
+    for t, name in ((q, "q"), (k_nope, "k_nope"), (k_pe, "k_pe"), (v, "v")):
+        _require(t.dtype == torch.bfloat16, f"{who}: {name} must be bfloat16")
+    for t, name in ((cu_seqlens_q, "cu_seqlens_q"), (cu_seqlens_kv, "cu_seqlens_kv")):
+        _require(t.dtype == torch.int32 and t.dim() == 1 and t.is_contiguous(),
+                 f"{who}: {name} must be contiguous int32 [num_batch + 1]")
+    num_batch = cu_seqlens_q.numel() - 1
+    _require(num_batch >= 1 and cu_seqlens_kv.numel() == num_batch + 1,
+             f"{who}: cu_seqlens_q and cu_seqlens_kv must both have num_batch + 1 >= 2 entries")
+    _require(q.dim() == 3 and q.size(2) == _MLA_PREFILL_DQK, f"{who}: q must be [total_q, H, 192]")
+    total_q, num_head = q.size(0), q.size(1)
+    _require(1 <= num_head <= 128, f"{who}: num heads must be 1..128")
+    _require(q.stride(2) == 1 and (num_head == 1 or q.stride(1) == _MLA_PREFILL_DQK),
+             f"{who}: q must be contiguous in (head, dim)")
+    _require(k_nope.dim() == 3 and tuple(k_nope.shape[1:]) == (num_head, _MLA_PREFILL_DV),
+             f"{who}: k_nope must be [total_kv, H, 128]")
+    _require(v.dim() == 3 and tuple(v.shape[1:]) == (num_head, _MLA_PREFILL_DV),
+             f"{who}: v must be [total_kv, H, 128]")
+    _require(k_pe.dim() == 2 and k_pe.size(1) == _MLA_PREFILL_DPE, f"{who}: k_pe must be [total_kv, 64]")
+    total_kv = k_nope.size(0)
+    _require(total_kv >= 1 and v.size(0) == total_kv and k_pe.size(0) == total_kv,
+             f"{who}: k_nope, k_pe and v must hold the same total_kv >= 1 tokens")
+    _require(k_nope.stride(2) == 1 and v.stride(2) == 1 and k_pe.stride(1) == 1,
+             f"{who}: k_nope, k_pe and v rows must be contiguous")
+    for t, name in ((q, "q"), (k_nope, "k_nope"), (k_pe, "k_pe"), (v, "v"),
+                    (cu_seqlens_q, "cu_seqlens_q"), (cu_seqlens_kv, "cu_seqlens_kv")):
+        _require(t.is_cuda and t.device == q.device, f"{who}: {name} must be a cuda tensor on q's device")
+    y = output
+    if y is None:
+        y = torch.empty((total_q, num_head, _MLA_PREFILL_DV), dtype=torch.bfloat16, device=q.device)
+    else:
+        _require(y.is_cuda and y.device == q.device and y.dtype == torch.bfloat16,
+                 f"{who}: output must be bfloat16 on q's device")
+        _require(y.is_contiguous() and tuple(y.shape) == (total_q, num_head, _MLA_PREFILL_DV),
+                 f"{who}: output must be contiguous [total_q, H, 128]")
+
+    def st(t, i, unit):
+        # the stride of a size-1 dim is never applied, and torch may report any value for it
+        return t.stride(i) if t.size(i) > 1 else unit
+
+    _check_rc(_lib.hpc_attention_prefill_mla_bf16_async(
+        _ptr(y), _ptr(q), _ptr(k_nope), _ptr(k_pe), _ptr(v), _ptr(cu_seqlens_q), _ptr(cu_seqlens_kv),
+        num_batch, total_q, total_kv, int(max_seqlen_q), num_head, q.size(2), v.size(2),
+        num_head * _MLA_PREFILL_DV, st(q, 0, num_head * _MLA_PREFILL_DQK),
+        st(k_nope, 0, num_head * _MLA_PREFILL_DV), st(k_nope, 1, _MLA_PREFILL_DV),
+        st(k_pe, 0, _MLA_PREFILL_DPE), st(v, 0, num_head * _MLA_PREFILL_DV), st(v, 1, _MLA_PREFILL_DV),
+        float(softmax_scale), _stream_of(q)), who)
+    return y
+
+
 # schemas of reference src/attention/entry.cc (attention_prefill_bf16,
 # attention_with_kvcache_prefill_bf16 registrations)
 _ops.define(
@@ -521,6 +580,12 @@ _ops.define(
     "Tensor cu_seqlens_q, Tensor block_ids, Tensor num_seq_kvcache, int max_seqlens_q, "
     "Tensor? output) -> (Tensor)")
 _ops.impl("attention_with_kvcache_prefill_bf16", _attention_with_kvcache_prefill_bf16_impl, "CUDA")
+
+_ops.define(
+    "attention_prefill_mla_bf16(Tensor q, Tensor k_nope, Tensor k_pe, Tensor v, "
+    "Tensor cu_seqlens_q, Tensor cu_seqlens_kv, int max_seqlen_q, float softmax_scale, "
+    "Tensor? output) -> (Tensor)")
+_ops.impl("attention_prefill_mla_bf16", _attention_prefill_mla_bf16_impl, "CUDA")
 
 _ops.define(
     "attention_decode_bf16(Tensor q, Tensor! kcache, Tensor! vcache, Tensor block_ids, Tensor "
@@ -653,6 +718,42 @@ def attention_with_kvcache_prefill_bf16(
     Returns bf16 [total_seq, num_head_q, 128]. Requests with sq = 0 write nothing."""
     return torch.ops.hpc.attention_with_kvcache_prefill_bf16(
         q, kcache, vcache, cu_seqlens_q, block_ids, seqlens_kvcache, max_seqlens_q, output)
+
+
+def attention_prefill_mla_bf16(
+    q: Tensor,
+    k_nope: Tensor,
+    k_pe: Tensor,
+    v: Tensor,
+    cu_seqlens_q: Tensor,
+    cu_seqlens_kv: Tensor,
+    max_seqlen_q: int,
+    softmax_scale: float,
+    output: Tensor = None,
+) -> Tensor:
+    """Multi-head latent attention (MLA) prefill in the un-absorbed form, varlen and causal.
+
+      q           [total_q, H, 192] bfloat16: per head q_nope (128) then the RoPE'd q_pe (64);
+                  contiguous in (head, dim), token stride a multiple of 8 elements. 1 <= H <= 128.
+      k_nope, v   [total_kv, H, 128] bfloat16, e.g. kv[..., :128] and kv[..., 128:] of a
+                  kv_b_proj output [total_kv, H, 256]
+      k_pe        [total_kv, 64] bfloat16, the RoPE'd key all heads share, e.g. latent[:, 512:] of
+                  a [total_kv, 576] latent buffer
+                  (k_nope, v and k_pe: any token and head strides that are multiples of 8
+                  elements, contiguous rows, 16-byte aligned; no copy is made)
+      cu_seqlens_q, cu_seqlens_kv  [B + 1] int32: request b has nq = cu_seqlens_q[b+1] -
+                  cu_seqlens_q[b] queries and nk = cu_seqlens_kv[b+1] - cu_seqlens_kv[b] keys
+      max_seqlen_q  at least the longest nq (a larger value only costs idle work items)
+      softmax_scale  used as given: s = (q_nope . k_nope + q_pe . k_pe) * softmax_scale
+                  (DeepSeek-V3: mscale^2 / sqrt(192))
+      output      optional contiguous bf16 [total_q, H, 128]
+    Causal masking is bottom-right: query i of request b sees its keys j <= nk - nq + i. So
+    cu_seqlens_kv == cu_seqlens_q is causal self-attention, and nk > nq is chunked prefill over a
+    prefix. Returns bf16 [total_q, H, 128]; a query that sees no key (nk < nq) gets zeros, and
+    rows of requests with nq = 0 are not written. The launch never synchronises, so it can be
+    captured in a CUDA graph."""
+    return torch.ops.hpc.attention_prefill_mla_bf16(
+        q, k_nope, k_pe, v, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, float(softmax_scale), output)
 
 
 def attention_decode_bf16(
@@ -932,3 +1033,11 @@ def _attention_with_kvcache_prefill_bf16_fake(q, kcache, vcache, cu_seqlens_q, b
         return output
     return torch.empty((q.size(0), q.size(1), vcache.size(3)), dtype=torch.bfloat16,
                        device=q.device)
+
+
+@torch.library.register_fake("hpc::attention_prefill_mla_bf16")
+def _attention_prefill_mla_bf16_fake(q, k_nope, k_pe, v, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q,
+                                     softmax_scale, output=None):
+    if output is not None:
+        return output
+    return q.new_empty((q.size(0), q.size(1), _MLA_PREFILL_DV))

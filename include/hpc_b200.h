@@ -454,6 +454,29 @@ int hpc_attention_with_kvcache_prefill_bf16_async(
     int ldQ, int64_t ldK, int64_t ldK1, int64_t ldK2, int64_t ldV, int64_t ldV1, int64_t ldV2,
     cudaStream_t stream);
 
+/* ---- prefill attention: MLA in the un-absorbed form (DeepSeek-V2/V3-style), bf16 ----------------
+ * y[t, h, :] = softmax_j(s_j) . v[kv0 + j, h, :] over the visible keys j of t's request, with
+ * s_j = (q[t, h, :128] . k_nope[kv0 + j, h, :] + q[t, h, 128:] . k_pe[kv0 + j, :]) * softmax_scale.
+ * Request b has nq = cu_seqlens_q[b+1] - cu_seqlens_q[b] queries (rows cu_seqlens_q[b] .. of q and
+ * y) and nk = cu_seqlens_kv[b+1] - cu_seqlens_kv[b] keys (rows kv0 = cu_seqlens_kv[b] .. of k_nope,
+ * k_pe and v); query i sees keys j <= nk - nq + i (bottom-right causal). A query that sees no key
+ * (nk < nq) gets a row of zeros; rows of requests with nq = 0 are not written.
+ *   q      [total_seq_q, H, 192] bf16, [q_nope (128) | q_pe (64)] per head, heads 192 apart,
+ *          token stride ldQ;  num_dim_qk must be 192, num_dim_v 128, 1 <= H <= 128
+ *   k_nope [total_seq_kv, H, 128], v [total_seq_kv, H, 128]: any token / head strides
+ *   k_pe   [total_seq_kv, 64], shared by all heads: any token stride
+ *   y      [total_seq_q, H, 128] bf16, heads 128 apart, token stride ldY
+ * Strides in elements, positive multiples of 8; every base 16-byte aligned; softmax_scale finite
+ * and positive, used as given. max_seq_q >= the longest request's nq. No allocation and no host
+ * synchronisation: capturable in a CUDA graph, and graphs may be replayed on several streams. */
+int hpc_attention_prefill_mla_bf16_async(
+    void* y_ptr, const void* q_ptr, const void* k_nope_ptr, const void* k_pe_ptr,
+    const void* v_ptr, const int* cu_seqlens_q_ptr, const int* cu_seqlens_kv_ptr, int num_batch,
+    int total_seq_q, int total_seq_kv, int max_seq_q, int num_head, int num_dim_qk, int num_dim_v,
+    int ldY, int ldQ, int64_t k_nope_token_stride, int64_t k_nope_head_stride,
+    int64_t k_pe_token_stride, int64_t v_token_stride, int64_t v_head_stride, float softmax_scale,
+    cudaStream_t stream);
+
 /* ---- RoPE + QK RMSNorm + paged KV-cache store (the producer of the cache layout attention reads) --
  * replaces reference src/rope/rope.h:15-25 (rope_norm_store_kv_async) and :27-38
  * (rope_norm_store_kv_fp8_async), argument for argument (bool -> int). Cache pages are

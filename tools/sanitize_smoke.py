@@ -1,7 +1,8 @@
 """One small invocation of every hot-path op (decode both quant types, prefill both, bf16 prefill
 dense and paged, blockwise + per-tensor MoE, bf16 MoE, route GEMM, allreduce with a simulated
 peer (P2P high-throughput, Lamport one-shot and two-shot), rope, the Stem mask stages,
-fused RMSNorm -> FP8, the masked activation quantisers and the speculative sampler),
+fused RMSNorm -> FP8, the masked activation quantisers, the speculative sampler and MLA decode and
+prefill),
 meant to run under compute-sanitizer:
 
     compute-sanitizer --tool memcheck  python tools/sanitize_smoke.py
@@ -29,7 +30,8 @@ def cuda(d):
 
 def main():
     which = set(sys.argv[1:]) or {"decode", "prefill", "prefill_bf16", "moe", "moe_bf16", "gemm",
-                                  "allreduce", "rope", "stem", "norm_act", "spec", "mla"}
+                                  "allreduce", "rope", "stem", "norm_act", "spec", "mla",
+                                  "mla_prefill"}
     if "decode" in which:
         B, hkv, hq = 3, 2, 8
         lens = [300, 129, 64]
@@ -265,6 +267,17 @@ def main():
         r = oml.check(y.float().cpu(), d)
         assert r["ok_a"] and r["ok_b"], r
         print("mla ok")
+    if "mla_prefill" in which:
+        # MLA prefill: two ragged requests, one over a prefix, NaN past the last key
+        from oracle import prefill_mla as omp
+        from synth import prefill_mla as smp
+        d = smp.make_case([130, 70], [300, 70], 4, seed=1, kind="edge")
+        y = hpc.attention_prefill_mla_bf16(d["q"].cuda(), d["k_nope"].cuda(), d["k_pe"].cuda(),
+                                           d["v"].cuda(), d["cu_seqlens_q"].cuda(),
+                                           d["cu_seqlens_kv"].cuda(), d["max_q"], d["scale"])
+        r = omp.check(y.float().cpu(), d)
+        assert r["ok_a"] and r["ok_b"], r
+        print("mla_prefill ok")
     torch.cuda.synchronize()
     print("smoke ok")
 
