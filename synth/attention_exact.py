@@ -94,10 +94,18 @@ def _needle_positions(n, sq, rows, gen, page=PAGE, front=None, rotate=0):
 
 
 def make_decode_exact_inputs(kind, lens, num_seq_q, num_head_kv, num_head_q, k_per_token=False,
-                             temperature=4.0, layout="NHD", seed=0, device="cpu"):
+                             temperature=4.0, layout="NHD", seed=0, device="cpu", seams=None,
+                             heads=None, climb=0.0):
     """Decode inputs in the format of synth.decode.make_decode_fp8_inputs (kv per tensor) or
     make_decode_fp8_kpt_inputs (k per token). kind: "peaked", "needle" or "kscale" (k per
-    token only). lens include the num_seq_q new tokens."""
+    token only). lens include the num_seq_q new tokens.
+
+    Needle kind, for the rotated bin walk (oracle.decode_walk): `seams` {(b, h): keys} puts the
+    needles of the rows of pair (b, h) on those keys first (decode_walk.seam_keys: both sides of
+    every seam, segment ends, tasks between save and restore), and `heads` {(b, h): [(first,
+    seam, end)]} with `climb` c adds c to the score of every key of the head part [first, seam)
+    of each split task, for all rows of the group: c > 0 puts the head part's maximum above the
+    tail's, c < 0 below it, so a restore that rescales m, l or O wrongly moves the output."""
     gen = torch.Generator().manual_seed(seed)
     lens = [int(n) for n in lens]
     B, sq, hkv, hq = len(lens), num_seq_q, num_head_kv, num_head_q
@@ -117,13 +125,18 @@ def make_decode_exact_inputs(kind, lens, num_seq_q, num_head_kv, num_head_q, k_p
         for b, n in enumerate(lens):
             dirs = H[(b % 4) * 32:(b % 4) * 32 + rows]
             nxt = H[((b + 1) % 4) * 32:((b + 1) % 4) * 32 + rows].sum(0) if B > 1 else None
+            shared = H[(b % 4) * 32 + 31]  # orthogonal to dirs (rows < 32) and to nxt
             page = ids[b].long()
             for h in range(hkv):
                 kv = kf[page, :, h].reshape(-1, D)  # this request's keys, a copy
+                ranges = (heads or {}).get((b, h), []) if climb else []
                 for r in range(rows):
                     gi, i = divmod(r, sq)
-                    qf[b, i, h * g + gi] = dirs[r]
-                pos = _needle_positions(n, sq, rows, gen)
+                    qf[b, i, h * g + gi] = dirs[r] + (shared if ranges else 0)
+                for lo, seam, _ in ranges:
+                    kv[lo:seam] += climb * shared / math.sqrt(D)
+                front = seams.get((b, h)) if seams is not None else None
+                pos = _needle_positions(n, sq, rows, gen, front=front)
                 for r in range(rows):
                     gi, i = divmod(r, sq)
                     kv[pos[r]] += (math.log(n) + 3.0) * dirs[r] / math.sqrt(D)

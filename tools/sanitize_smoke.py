@@ -1,8 +1,8 @@
 """One small invocation of every hot-path op (decode both quant types, prefill both, bf16 prefill
 dense and paged, blockwise + per-tensor MoE, bf16 MoE, route GEMM, allreduce with a simulated
 peer (P2P high-throughput, Lamport one-shot and two-shot), rope, the Stem mask stages,
-fused RMSNorm -> FP8, the masked activation quantisers, the speculative sampler and MLA decode and
-prefill),
+fused RMSNorm -> FP8, the masked activation quantisers, the speculative sampler, MLA decode and
+prefill, and a multi-row split of the rotated decode walk in the FP8 and MLA decode kernels),
 meant to run under compute-sanitizer:
 
     compute-sanitizer --tool memcheck  python tools/sanitize_smoke.py
@@ -31,7 +31,7 @@ def cuda(d):
 def main():
     which = set(sys.argv[1:]) or {"decode", "prefill", "prefill_bf16", "moe", "moe_bf16", "gemm",
                                   "allreduce", "rope", "stem", "norm_act", "spec", "mla",
-                                  "mla_prefill"}
+                                  "mla_prefill", "walk"}
     if "decode" in which:
         B, hkv, hq = 3, 2, 8
         lens = [300, 129, 64]
@@ -267,6 +267,46 @@ def main():
         r = oml.check(y.float().cpu(), d)
         assert r["ok_a"] and r["ok_b"], r
         print("mla ok")
+    if "walk" in which:
+        # the rotated bin walk (oracle/decode_walk.py): one multi-row split call for each kernel
+        from oracle import attention_mla as oml
+        from oracle import decode_walk as dw
+        from synth import attention_mla as sml
+        from synth.attention_exact import make_decode_exact_inputs
+        ctas = hpc._ffi.sm_count()
+        for kind, T, sq, h in (("fp8", 2, 1, 8), ("mla", 2, 1, 128)):
+            lens = [2000 + 347 * i for i in range(12)]
+            walks = dw.walk(dw.task_map(lens, ctas, T, sq, 64), len(lens), T)
+            assert dw.path_counts(walks, sq).get("d"), "no multi-row split walk"
+            dlens = torch.tensor(lens, dtype=torch.int32, device="cuda")
+            tm = hpc.get_attention_decode_task_workspace(len(lens), max(lens) + sq, T, 64)
+            hpc.assign_attention_decode_task(dlens, tm, T, sq, True, 64)
+            if kind == "fp8":
+                d = make_decode_exact_inputs("needle", lens, sq, T, h, seams=dw.seam_keys(walks),
+                                             seed=5)
+                c = cuda(d)
+                y = hpc.attention_decode_fp8(c["q"], c["kvcache"][:, 0], c["kvcache"][:, 1],
+                                             c["block_ids"], dlens, c["q_scale"], c["k_scale"],
+                                             c["v_scale"], mtp=0, new_kv_included=True,
+                                             quant_type=hpc.QuantType.QPERTOKEN_PERHEAD_KPERTENSOR_VPERTENSOR,
+                                             splitk=True, task_map=tm)
+                from oracle import attention_exact as ox
+                k, v = d["kvcache"][:, 0], d["kvcache"][:, 1]
+                ex, bnd = ox.decode_fp8_exact(d["q"], k, v, d["block_ids"], d["kv_lens_total"],
+                                              d["q_scale"], d["k_scale"], d["v_scale"], sq)
+                lossy = oa.decode_fp8_kvpertensor(d["q"], k, v, d["block_ids"], d["kv_lens_total"],
+                                                  d["q_scale"], d["k_scale"], d["v_scale"], sq)
+                ox.assert_exact(y.cpu(), ex, bnd, lossy, "walk fp8")
+            else:
+                d = sml.make_case(lens, h, 0, seed=5, kind="needle", num_total_ctas=ctas,
+                                  min_process_len=64, seams=dw.seam_keys(walks))
+                y = hpc.attention_decode_mla_bf16(d["q"].cuda(), d["kv"].cuda(), d["block_ids"].cuda(),
+                                                  dlens, d["scale"], mtp=0, new_kv_included=True,
+                                                  task_map=tm)
+                r = oml.check(y.float().cpu(), d)
+                assert r["ok_a"] and r["ok_b"], r
+            torch.cuda.synchronize()
+        print("walk ok")
     if "mla_prefill" in which:
         # MLA prefill: two ragged requests, one over a prefix, NaN past the last key
         from oracle import prefill_mla as omp
